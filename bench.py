@@ -2,6 +2,7 @@
 """Benchmark of the Chebyshev filtering hot path (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+                    [--dump-outputs DIR]
 
 metric  = cheby_op filtered-vertices/sec = N * Nsig * order / t
 workload, 1 GPU : BASELINE configs[1] -- Sensor-type 2-D k-NN graph, N = 1e6, k = 10,
@@ -26,10 +27,15 @@ roofline: algorithmic bytes of the recurrence / measured kernel time vs the
           measured HBM copy bandwidth (MEASURED_PEAKS.json).
 cpu_baseline: the unmodified reference (baseline/_ref; the oracle port if absent) on one core,
           a bounded sample of the same workload.
+--dump-outputs DIR: after the timed steps, DIR/y.npy (DIR/y_rank<r>.npy on N > 1) holds what
+          the last timed call returned, (Nscales, rows, Nsig) float32: every row when the
+          block fits DUMP_BYTES, else a fixed seeded sample of rows (the same rows on every run
+          with the same arguments), so that two builds can be compared output for output.
 --impl reference: the unmodified reference's CPU path on up to 64 host processes
           (one signal column each; the reference is single-threaded by construction).
 """
 import argparse
+import atexit
 import json
 import os
 import subprocess
@@ -80,6 +86,8 @@ def parse():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--cpu-columns", type=int, default=4)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed call's result (or a seeded row sample) as .npy")
     return ap.parse_args()
 
 
@@ -128,7 +136,7 @@ def config_dict(wl, world, scaling):
                          "1-D vertex partition, %d contiguous row blocks, halo exchange per "
                          "recurrence step" % world,
             "l2_policy": "inputs_exceed_l2 (the state blocks of a call are >= 0.5 GB per GPU, "
-                         "L2 is 126 MB)"}
+                         "L2 is 50 MB)"}
 
 
 def pick_workload(args, world):
@@ -221,7 +229,7 @@ def measured_peak():
             return float(json.load(open(path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet HBM3 bandwidth (3.35 TB/s), not measured"
 
 
 def ncu_traffic(workload):
@@ -244,9 +252,9 @@ REF_DIR = os.path.join(ROOT, "baseline", "_ref")
 
 
 def _import_reference():
-    """The unmodified PyGSP 0.6.1, pip-installed offline into baseline/_ref (git-ignored,
-    travels with the snapshot): `pip install --no-index --no-deps --target baseline/_ref
-    /root/reference`.  None when absent -- the oracle port then stands in."""
+    """The unmodified PyGSP 0.6.1, pip-installed offline into baseline/_ref (git-ignored):
+    `pip install --no-index --no-deps --target baseline/_ref <PyGSP 0.6.1 source tree>`.
+    None when absent -- the oracle port then stands in."""
     if not os.path.isdir(os.path.join(REF_DIR, "pygsp")):
         return None
     if REF_DIR not in sys.path:
@@ -406,6 +414,22 @@ def time_calls(torch, fn, x, steps, warm):
     return start.elapsed_time(stop) / steps
 
 
+DUMP_BYTES = 48 << 20         # --dump-outputs: at most this many bytes over all ranks
+
+
+def dump_outputs(torch, out_dir, y, rank, world):
+    """Write y ((Nscales, n, Nsig) device tensor) as float32 .npy: whole, or the rows of a
+    default_rng(0) sample (sorted) when it exceeds this rank's share of DUMP_BYTES."""
+    nscales, n, nsig = y.shape
+    rows = max(1, DUMP_BYTES // world // (4 * nscales * nsig))
+    if rows < n:
+        pick = np.sort(np.random.default_rng(0).choice(n, size=rows, replace=False))
+        y = y[:, torch.from_numpy(pick).to(y.device), :]
+    os.makedirs(out_dir, exist_ok=True)
+    name = "y.npy" if world == 1 else "y_rank%d.npy" % rank
+    np.save(os.path.join(out_dir, name), y.float().cpu().numpy())
+
+
 def oracle_parity(L, lmax, c, x_col, got):
     """max|got - ref| / max|ref| of one signal column against the float64 oracle (CPU)."""
     from oracle import pygsp_oracle as orc
@@ -518,6 +542,22 @@ def build_partitioned_from_graph(G, rank, world, torch):
     return op, (lo, hi)
 
 
+def native_library(gsp):
+    """The package's library as build() left it.  The tree may be read-only here, and a package
+    whose build() always takes its lock (a file next to the library) cannot load from such a
+    tree; there a library whose stamp matches the sources is loaded without the lock, and a
+    missing or stale one is an error (nothing may be rebuilt in a read-only tree)."""
+    b = gsp._native._build
+    if not os.access(b.OUT_DIR, os.W_OK):
+        stamp = os.path.join(b.OUT_DIR, "stamp.txt")
+        if not (os.path.exists(b.LIB) and os.path.exists(stamp)
+                and open(stamp).read().strip() == b._stamp()):
+            raise SystemExit("%s is missing or older than its sources, and the tree is read-only:"
+                             " run build() first" % b.LIB)
+        b.build = lambda force=False, verbose=False: b.LIB
+    return gsp._native.lib()
+
+
 def run_ours(args):
     import ctypes
     import torch
@@ -537,12 +577,13 @@ def run_ours(args):
     nsig, order = wl["nsig"], wl["order"]
     if world > 1 and name == "config3":
         raise SystemExit("--workload config3 is a single-GPU option")
-    lib = gsp._native.lib()
+    lib = native_library(gsp)
     lib.gsp_launch_count.restype = ctypes.c_uint64
     peak, peak_src = measured_peak()
 
     clocks = ClockSampler(local)
     clocks.__enter__()                       # running long before the timed region
+    atexit.register(clocks.__exit__)         # stopped even when the run fails
 
     def barrier():
         if world > 1:
@@ -628,6 +669,8 @@ def run_ours(args):
     clocks.__exit__()
     t_dev = allmax(start.elapsed_time(stop) / 1e3)
     value = n_global * nsig * order * args.steps / t_dev
+    if args.dump_outputs:
+        dump_outputs(torch, args.dump_outputs, y_dev, rank, world)
 
     # ---- end to end through the public API with host buffers
     e2e = None

@@ -1,4 +1,4 @@
-/* libgspb200 -- C ABI of the B200-native Chebyshev graph-filtering engine.
+/* libgspb200 -- C ABI of the H100-native Chebyshev graph-filtering engine.
  *
  * The reference (PyGSP 0.6.1) has no FFI: its seam for this path is the Python
  * call boundary, below which every operation is a call into SciPy's compiled
@@ -86,7 +86,7 @@ int gsp_cheby_tile_plan(int64_t n, const int32_t* indptr, int64_t nsig, int nsca
  * peer_flags[q] when the last front tile is done -- at that point the pushed rows are visible
  * and nobody on this GPU reads the halo of x_cur any more, so the neighbours may also
  * overwrite it.  Then all interior tiles, with the plain kernel instantiation (one kernel
- * for both spilled registers into the interior loop: 1.6 x slower steps).  All pointers are
+ * for both spills registers into the interior loop and runs slower).  All pointers are
  * device pointers; the struct itself is a host struct.  n_push_tiles / n_wait_tiles are
  * filled in by the library. */
 typedef struct gsp_halo_fusion {

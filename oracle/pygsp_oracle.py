@@ -7,7 +7,7 @@ thing measured as the product or shipped.
 
 Parity status: PINNED.  ``tests/test_oracle_golden.py`` checks every function
 below against fixtures under ``tests/golden/`` that were produced by importing
-the real reference (``/root/reference``, PyGSP 0.6.1 @ 4716b12) with
+the real reference (PyGSP 0.6.1 @ 4716b12) with
 ``tests/golden/make_golden.py`` -- the Logo README example, the
 ``Sensor(123, seed=42)`` fixtures of the reference's own test-suite, the
 Laplacian / lmax known-answer matrices of ``pygsp/tests/test_graphs.py`` and

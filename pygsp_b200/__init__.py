@@ -1,8 +1,8 @@
-"""pygsp_b200 -- Blackwell-native Chebyshev spectral graph filtering.
+"""pygsp_b200 -- Hopper-native Chebyshev spectral graph filtering.
 
 Drop-in for the ``Graph.compute_laplacian`` -> ``Graph.estimate_lmax`` ->
 ``Filter.filter(method='chebyshev')`` -> ``approximations.cheby_op`` path of
-PyGSP 0.6.1, computed by hand-written sm_100a CUDA kernels (``libgspb200.so``)
+PyGSP 0.6.1, computed by hand-written sm_90a CUDA kernels (``libgspb200.so``)
 behind the reference's Python API.  There is no CPU fallback.
 """
 from . import _native  # noqa: F401

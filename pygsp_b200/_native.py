@@ -149,5 +149,5 @@ def stream_ptr(device=None):
 def require_cuda():
     import torch
     if not torch.cuda.is_available():
-        raise NativeError("pygsp_b200 needs a CUDA device (B200): there is no CPU fallback")
+        raise NativeError("pygsp_b200 needs a CUDA device (H100): there is no CPU fallback")
     return torch

@@ -1,4 +1,4 @@
-"""Builds libgspb200.so in-tree with nvcc for sm_100a (no JIT, no torch extension)."""
+"""Builds libgspb200.so in-tree with nvcc for sm_90a (no JIT, no torch extension)."""
 import hashlib
 import os
 import shutil
@@ -11,7 +11,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT_DIR = os.path.join(HERE, "_lib")
 LIB = os.path.join(OUT_DIR, "libgspb200.so")
 SOURCES = ["runtime.cu", "cheby.cu", "cheby_tiled.cu", "graph.cu", "lanczos.cu", "halo.cu", "generate.cu", "staging.cu", "dist.cu", "cg.cu"]
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 
 def _nvcc():
@@ -31,11 +31,23 @@ def _stamp():
     return h.hexdigest()
 
 
+def is_current():
+    """True when the library exists and was built from the sources as they are."""
+    stamp_file = os.path.join(OUT_DIR, "stamp.txt")
+    if not (os.path.exists(LIB) and os.path.exists(stamp_file)):
+        return False
+    with open(stamp_file) as fh:
+        return fh.read().strip() == _stamp()
+
+
 def build(force=False, verbose=False):
-    """Build (if the sources changed) and return the path of the library.  One process at a
-    time (flock on _lib/.lock: torchrun starts one process per GPU on the same tree); objects
-    and the library are written under temporary names and renamed into place."""
+    """Build (if the sources changed) and return the path of the library.  A current library
+    is returned without writing anything (the tree may be read-only once built).  Otherwise one
+    process at a time (flock on _lib/.lock: torchrun starts one process per GPU on the same
+    tree); objects and the library are written under temporary names and renamed into place."""
     import fcntl
+    if not force and is_current():
+        return LIB
     os.makedirs(OUT_DIR, exist_ok=True)
     with open(os.path.join(OUT_DIR, ".lock"), "w") as lock:
         fcntl.flock(lock, fcntl.LOCK_EX)
@@ -48,9 +60,8 @@ def build(force=False, verbose=False):
 def _build_locked(force, verbose):
     stamp_file = os.path.join(OUT_DIR, "stamp.txt")
     stamp = _stamp()
-    if not force and os.path.exists(LIB) and os.path.exists(stamp_file):
-        if open(stamp_file).read().strip() == stamp:
-            return LIB
+    if not force and is_current():       # another process built it while this one waited
+        return LIB
     nvcc = _nvcc()
     objs = []
     procs = []

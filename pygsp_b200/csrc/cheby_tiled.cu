@@ -1,4 +1,4 @@
-// Tiled, warp-specialised Chebyshev step for sm_100a: the float32 fast path.
+// Tiled, warp-specialised Chebyshev step for sm_90a: the float32 fast path.
 //
 // Same arithmetic as cheby_step_rowgroup (csrc/cheby.cu) -- and therefore the same
 // reference lines, pygsp/filters/approximations.py:99-112 -- but every operand
@@ -356,7 +356,7 @@ __device__ __forceinline__ void tile_rows(const TileArgs& a, const TileCtx t) {
 // A boundary ("front") tile of a partitioned step -- a few tiles per launch.  It is a real
 // function call on purpose: inlined, its extra state (flags, peer tables, a second copy of
 // the gather loop) made ptxas spill registers in the interior tiles' loop as well
-// (1.6 x slower steps, measured).  Does, for one consumer warp:
+// (slower steps).  Does, for one consumer warp:
 //   wait   : until the neighbours have published the halo of x_cur (they stored it straight
 //            into this GPU's memory and released wait_value afterwards);
 //   rows   : the tile's rows with coherent gathers;
@@ -721,12 +721,12 @@ int cheby_step_tiled_f32(bool first, int64_t rb, int64_t re, int64_t nnz, const 
   const bool h = halo != nullptr;
   // two packets per lane (32 / 64 / 128 signals): a CSR read in shared memory serves twice
   // as many rows; GSPB200_TILE_P2=0 / 1 forces one / two packets per lane.
-  // Measured (profiles/r2_probe_p2_*.jsonl, Clenshaw form with direct vector loads): 64 signals
-  // 8.13 -> 6.97 ms per order-30 call, 128 signals 15.9 -> 12.6 ms, 32 signals 4.80 -> 4.73 ms;
-  // the forward recurrence with TMA-staged vectors is slower with it (8.8 -> 9.3 ms: only two of
-  // the three CTAs fit), so the default follows the form.
-  const bool two = !h && nsig >= 32 &&
-                   env_int("GSPB200_TILE_P2", (a.add_source && a.vec_direct) ? 1 : 0) != 0;
+  // Measured on an H100 SXM (400 W limit), 1e6-vertex graphs, interleaved A/B, one -> two packets:
+  // Clenshaw form (direct vectors), order 30: 64 signals 18.4 -> 15.7 ms per call, 128 signals
+  // 38.0 -> 31.6 ms, 32 signals 10.2 -> 8.9 ms; forward form (TMA-staged vectors): one filter at
+  // 64 signals 23.5 -> 19.2 ms, two filters 29.2 / 30.8 -> 27.6 / 27.3 ms, a 6-filter MexicanHat
+  // bank at order 50 on a grid 89.8 / 97.1 -> 84.0 / 84.1 ms.  So two packets are the default.
+  const bool two = !h && nsig >= 32 && env_int("GSPB200_TILE_P2", 1) != 0;
   if (two) a.consumer_warps = std::min(a.consumer_warps, 8);
   switch (nsig) {
     case 8: return launch_tiled_g<2>(first, a, h, false, plan.blocks_per_sm, st);
@@ -742,9 +742,9 @@ int cheby_step_tiled_f32(bool first, int64_t rb, int64_t re, int64_t nnz, const 
 // (1) The boundary ("front") tiles -- those holding rows that read halo columns or that some
 // neighbour needs -- with the halo-capable instantiation: wait for the neighbours' flags, coherent
 // gathers, peer stores of the new boundary rows, publish.  (2) All interior tiles with the plain
-// instantiation.  One kernel for both was 1.6 x slower per step (DESIGN.md section 5): under the
-// 60-register cap ptxas spilled the boundary code's state inside the interior gather loop.  The
-// front launch is a few dozen tiles (~10 us) and publishes before the interior tiles run, so the
+// instantiation.  One kernel for both is slower per step (DESIGN.md section 5): under the
+// 60-register cap ptxas spills the boundary code's state inside the interior gather loop.  The
+// front launch is a few dozen tiles and publishes before the interior tiles run, so the
 // neighbours' next front launch finds the flag set.  Reports the rows done (whole tiles).
 int cheby_step_tiled_halo_f32(bool first, int64_t n, int64_t nnz, const int32_t* indptr,
                               const int32_t* indices, const float* vals, const float* x_cur,

@@ -1,4 +1,4 @@
-// Shared helpers for libgspb200 (sm_100a only).
+// Shared helpers for libgspb200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

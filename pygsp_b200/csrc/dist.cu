@@ -80,9 +80,9 @@ static int dist_step(const gsp_dist_plan* p, const gsp_tile_plan* tile, bool fus
     // Two launches on the same stream.  (1) The boundary ("front") tiles with the
     // halo-capable instantiation: wait for the neighbours' flags, coherent gathers, peer
     // stores of the new boundary rows, publish.  (2) All interior tiles with the plain
-    // instantiation.  One kernel for both was 1.6 x slower per step: the boundary code's
-    // registers spilled inside the interior tiles' gather loop (ptxas, 60-register cap);
-    // the front launch is a few dozen tiles (~10 us) and publishes before the interior runs.
+    // instantiation.  One kernel for both is slower per step: the boundary code's registers
+    // spill inside the interior tiles' gather loop (ptxas, 60-register cap); the front
+    // launch is a few dozen tiles and publishes before the interior runs.
     const int R = tile->rows_per_tile;
     const int64_t front_rows =
         ceil_div(std::max<int64_t>(publish ? p->n_push_rows : 0, p->n_boundary_rows), (int64_t)R) * R;

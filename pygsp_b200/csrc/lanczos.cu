@@ -70,8 +70,8 @@ __global__ void lanczos_seed_kernel(int64_t n, T* v, uint64_t seed, double* part
 // -- neighbours in memory -- share 128-byte lines), row sums reduced with warp shuffles
 // (graph.py:911-917 spends its time in exactly this product).
 //
-// What bounded the first version (ncu: 51 us for N = 1e6, nnz = 1.2e7 = 0.33 of HBM) was not
-// DRAM but the L1 tag stage: a warp's 32 scalar gathers x[col] touch ~16 different lines.  So a
+// What bounds a thread-per-row or warp-per-row product on such graphs is not DRAM but the L1
+// tag stage: a warp's 32 scalar gathers x[col] touch ~16 different lines.  So a
 // block owns a TILE of TR consecutive rows and keeps x[tile] and indptr[tile] in shared
 // memory: with a locality-preserving vertex numbering (Morton) ~90 % of a row's neighbours
 // lie inside its own tile and are served from shared memory (conflict-limited, a few cycles per
@@ -244,8 +244,8 @@ static inline int spmv_lanes_subwarp(int64_t n, int64_t nnz) {
   if (e && (atoi(e) == 2 || atoi(e) == 4 || atoi(e) == 8 || atoi(e) == 16 || atoi(e) == 32))
     return atoi(e);
   // about three entries per lane: fewer, longer lane chains and more rows in flight per warp beat
-  // one entry per lane (N = 1e6, 12.4 entries per row, L2-warm: 4 lanes 34 us, 8 lanes 49 us,
-  // 16 lanes 65 us -- profiles/r2_spmv_probe_b.jsonl)
+  // one entry per lane (N = 1e6, 12.4 entries per row, L2-warm on an H100 SXM at 400 W: 4 lanes
+  // 55-58 us, 16 lanes 70 us per product; tools/spmv_probe.py)
   const double mean = n > 0 ? double(nnz) / double(n) : 1.0;
   int lpr = 2;
   while (lpr < 32 && 3 * (2 * lpr) <= mean) lpr *= 2;

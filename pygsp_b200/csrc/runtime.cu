@@ -16,11 +16,11 @@ unsigned long long launches() { return __atomic_load_n(&g_launches, __ATOMIC_REL
 int sm_count() {
   static int cached[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (cached[dev] == 0) {
     int v = 0;
     if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0)
-      v = 148;
+      v = 132;
     cached[dev] = v;
   }
   return cached[dev];

@@ -1,6 +1,6 @@
 """Vertex-partitioned Chebyshev filtering: one process per GPU, halo exchange per step.
 
-The reference is single-process (SURVEY.md 8e); this is the B200 scale-out of
+The reference is single-process (SURVEY.md 8e); this is the multi-GPU scale-out of
 ``approximations.cheby_op`` (pygsp/filters/approximations.py:58-114).  The graph's
 vertices are split into P contiguous row blocks.  Rank p owns rows
 [bounds[p], bounds[p+1]) of L and the matching slices of T_{k-2}, T_{k-1} and r;
@@ -215,9 +215,9 @@ class PartitionedCheby:
         self.backend = backend if backend is not None else _CudaBackend(device)
         self.device = self.backend.device
         self.dtype = dtype if dtype is not None else torch.float32
-        # Splitting a step into boundary + interior launches costs ~30 us; it pays
-        # only when the exchange itself is long (measured on 2 x B200: a 0.4 MB
-        # halo is 3 % faster unsplit).  None = decide per call from the halo size.
+        # Splitting a step into boundary + interior launches costs launches and tile
+        # ramp-up; it pays only when the exchange itself is long (a sub-MB halo runs
+        # faster unsplit).  None = decide per call from the halo size.
         self.overlap = overlap
         self.overlap_min_bytes = 16 << 20
         self.p2p_max_halo_fraction = 0.25
@@ -313,9 +313,8 @@ class PartitionedCheby:
         n, nb = p.n_local, p.n_boundary
         ext = n + p.n_halo
         # Small halos (k-NN / grid cuts: < 1 MB): the exchange fused into the step kernel
-        # wins (7.58 vs 7.89 ms on 2 GPUs).  Huge halos (SBM: 588 MB per step): one packed
-        # NCCL transfer overlapped with the interior rows beats 128-byte peer stores
-        # (95.7 vs 109.2 ms).  Measured on 2 x B200, profiles/r1_bench_*n2*.json.
+        # wins.  Huge halos (SBM: hundreds of MB per step): one packed NCCL transfer
+        # overlapped with the interior rows beats 128-byte peer stores.
         mode = self._exchange_mode(nsig)
         if mode == "p2p":
             return self._cheby_op_p2p(lmax, c, x, local_order,

@@ -3,7 +3,7 @@
 ``Filter.filter`` / ``cheby_op`` take and return host arrays in the reference
 (pygsp/filters/filter.py:146-328, approximations.py:58-114).  Uploading the block,
 running the recurrence and downloading the result one after the other makes the two
-transfers longer than the recurrence itself (config 2: 4.7 + 7.9 + 4.7 ms).  The
+transfers longer than the recurrence itself (256 MB each way for config 2).  The
 recurrence needs all ROWS of its operand before its first step but its COLUMNS are
 independent, so the block is cut into column chunks and three streams run as a
 pipeline:
@@ -40,9 +40,9 @@ def chunk_plan(n, nsig, itemsize):
 
     Two halves: 64 signals -> 32 | 32.  Narrower chunks shorten the first upload and the last
     download, which overlap nothing, but every chunk re-reads the CSR arrays at every order and
-    narrow blocks run the recurrence less efficiently -- the pipeline is compute-bound, so the
-    halves win (config 2, one box: 16 | 32 | 16 -> 15.8 ms, 32 | 32 -> 14.8 ms, 4 x 16 -> 17.0 ms
-    per call; profiles/r2_e2e_trace.txt has the timelines).  The width must be one the
+    narrow blocks run the recurrence less efficiently -- the pipeline is compute-bound, so
+    quarters lose (config 2 on an H100 SXM at 400 W: 32 | 32 -> 25.3 ms, whole block 25.2 ms,
+    4 x 16 -> 27.7 ms per call; GSPB200_E2E_TRACE=1 records the timelines).  The width must be one the
     tiled kernel supports; blocks that are small (< 32 MB) or do not split that way are taken
     whole.  GSPB200_E2E_CHUNK=w forces equal chunks of w signals (0 = no pipelining)."""
     env = os.environ.get("GSPB200_E2E_CHUNK")

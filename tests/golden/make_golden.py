@@ -1,8 +1,8 @@
 """Generate the golden fixtures under tests/golden/ from the REAL reference.
 
-Run once in the build container (the reference cannot travel to the GPU box):
+Run once on any machine with a PyGSP 0.6.1 source tree (no GPU needed):
 
-    PYTHONPATH=/root/reference python tests/golden/make_golden.py
+    PYTHONPATH=<PyGSP 0.6.1 source tree> python tests/golden/make_golden.py
 
 Every array saved here is an output of unmodified PyGSP 0.6.1 code
 (`pygsp.graphs.Graph`, `pygsp.filters.*`, `pygsp.filters.approximations`).
@@ -13,12 +13,10 @@ start vector), and every consumer (oracle, CUDA engine) is given that value.
 
 import logging
 import os
-import sys
 
 import numpy as np
 from scipy import sparse
 
-sys.path.insert(0, "/root/reference")
 import pygsp  # noqa: E402
 from pygsp import filters, graphs  # noqa: E402
 from pygsp.filters import approximations  # noqa: E402

@@ -1,5 +1,5 @@
 """Golden fixtures for the callers of the filtering path (SURVEY.md 8f rank 3), from the REAL
-reference:  PYTHONPATH=/root/reference python tests/golden/make_golden_r2.py
+reference:  PYTHONPATH=<PyGSP 0.6.1 source tree> python tests/golden/make_golden_r2.py
 
   pyramid.npz  : pygsp.reduction.graph_multiresolution (levels=3, sparsify=False) of a
                  Sensor graph; per level W, lmax, mr['idx'], mr['K_reg']; outputs of
@@ -15,12 +15,10 @@ lmax values are computed once by the reference and stored (its ARPACK start vect
 """
 import logging
 import os
-import sys
 
 import numpy as np
 from scipy import sparse
 
-sys.path.insert(0, "/root/reference")
 import pygsp  # noqa: E402
 from pygsp import filters, graphs, learning, reduction  # noqa: E402
 

@@ -1,5 +1,5 @@
 """GPU parity tests: the CUDA path (through the C ABI) against the oracle and the
-golden fixtures generated from PyGSP 0.6.1.  Run on the B200 box: pytest -m gpu.
+golden fixtures generated from PyGSP 0.6.1.  Run on an H100: pytest -m gpu.
 
 Tolerances (BASELINE.json north_star / SURVEY.md 8c):
   * CSR indptr / indices of L: bit-exact;

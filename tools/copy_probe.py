@@ -1,4 +1,4 @@
-"""PCIe staging rates of column chunks of a row-major pinned (n, 64) float32 block (GPU box).
+"""PCIe staging rates of column chunks of a row-major pinned (n, 64) float32 block (needs a GPU).
 
     python tools/copy_probe.py [--n 1000000]
 

@@ -1,6 +1,6 @@
 """Per-kernel totals of an ncu launch list (`--metrics gpu__time_duration.sum --csv`).
 
-    python tools/launch_summary.py profiles/r2_launches.csv "command that was profiled" > profiles/r2_launches.summary.txt
+    python tools/launch_summary.py launches.csv "command that was profiled" > profiles/launches.summary.txt
 """
 import collections
 import csv

@@ -1,7 +1,7 @@
 """Summarise an .ncu-rep (read here, no GPU needed) into profiles/<name>.summary.txt and,
 with --traffic, profiles/roofline_traffic.json (DRAM bytes per launch of the dominant kernel).
 
-    python tools/ncu_summary.py profiles/r1_v1_tiled_step.ncu-rep [--traffic]
+    python tools/ncu_summary.py profiles/tiled_step.ncu-rep [--traffic]
 """
 import csv
 import io

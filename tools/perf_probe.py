@@ -1,8 +1,8 @@
-"""Interleaved A/B timing of the recurrence forms on the bench workload (run on the GPU box).
+"""Interleaved A/B timing of the recurrence forms on the bench workload (needs a GPU).
 
     python tools/perf_probe.py [--n 1000000] [--rounds 5] [--calls 10]
 
-Builds BASELINE config 2 once and times, round-robin in ONE process (so that box state,
+Builds BASELINE config 2 once and times, round-robin in ONE process (so that machine state,
 allocator state and clocks are shared): forward recurrence, Clenshaw form, and the same with
 GSPB200_* toggles flipped at run time (the library reads them per launch).  One JSON line per
 variant with every round's ms per call.

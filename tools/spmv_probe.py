@@ -1,9 +1,9 @@
-"""SpMV (Lanczos operator) timing on the bench graph, L2-warm and L2-cold (GPU box).
+"""SpMV (Lanczos operator) timing on the bench graph, L2-warm and L2-cold (needs a GPU).
 
     python tools/spmv_probe.py [--n 1000000]
 
 Variants are selected through GSPB200_SPMV / GSPB200_SPMV_TR (read per launch).  Warm: 50
-back-to-back products (x, indptr and most of the CSR stay in the 126 MB L2, as inside
+back-to-back products (x, indptr and most of the CSR stay in the 50 MB L2, as inside
 Lanczos); cold: a 512 MB memset between products.  One JSON line per variant.
 """
 import argparse

@@ -1,4 +1,4 @@
-"""Times Filter.filter synthesis (Nf features -> 1) fused vs reference order (GPU box)."""
+"""Times Filter.filter synthesis (Nf features -> 1) fused vs reference order (needs a GPU)."""
 import json
 import os
 import sys
