@@ -55,7 +55,11 @@ int gsp_device_info(int* sm_count, int* cc_major, int* cc_minor, int64_t* l2_byt
  *   single-filter evaluation; nsrc = Nf is the synthesis of filter.py:313-322 (which runs Nf
  *   forward recurrences).  out is (n, nsig), work 2*n*nsig.  Same value as the forward
  *   recurrence, different rounding.
- * gsp_spmm_*: y = L x, scipy `csr_matrix.dot` (approximations.py:99, graph.py:955).
+ * gsp_spmm_*: y = L x, scipy `csr_matrix.dot` (approximations.py:99, graph.py:955).  n is the
+ *   number of ROWS of the matrix; x is read at the column indices only, so the matrix may be
+ *   rectangular (n x m with x of m rows), as the differential operator's D and D^T are
+ *   (difference.py:244, 331).  gsp_spmv_* below is for square matrices only (its window form
+ *   stages x at the rows of its own tile).
  */
 /* Tiling of the float32 fast path (TMA-staged row tiles, csrc/cheby_tiled.cu).
  * Filled by gsp_cheby_tile_plan() once per (matrix, nsig, nscales); all zeros
@@ -410,6 +414,51 @@ int gsp_knn_to_csr_f64(int64_t n, int k, const int32_t* nn_idx, const double* nn
 
 GSPB200_DECLARE_GRAPH_API(f32, float)
 GSPB200_DECLARE_GRAPH_API(f64, double)
+
+/* -------------------------------------------------------- differential operator ---
+ * pygsp/graphs/difference.py:144-166 and graph.py:1019-1029, built on the device from a
+ * canonical CSR adjacency W (n x n).  Edges are numbered in row-major CSR order: the entries
+ * with col >= row (self-loops included) of an undirected W, every entry of a directed one.
+ * D is the n x Ne incidence matrix (CSR), Dt = D^T (Ne x n, CSR; its arrays are the CSC arrays
+ * of the reference's D).  A self-loop is an edge with an empty row of Dt (the reference's two
+ * entries cancel and eliminate_zeros() drops them), so nnz(D) = 2 (Ne - loops); the caller
+ * checks nnz(D) < 2^31 before allocating.  Values in double, rounded once: combinatorial
+ * -+sqrt(w), normalized -sqrt(w / dw[s]) / +sqrt(w / dw[t]), divided by sqrt(2) if directed.
+ * gsp_edge_offsets:     eptr (n + 1) = scan of each row's entries with col >= row (undirected;
+ *     a directed graph's edge offsets are W's indptr).
+ * gsp_edge_list_*:      sparse.triu(W, format='coo') / W.tocoo() (graph.py:1019-1026): sources,
+ *     targets (int32) and weights (n_edges each), and Dt's indptr (n_edges + 1).
+ * gsp_incidence_t_fill_*: Dt's indices / data (difference.py:147-166); dw (double) is the
+ *     weighted degree the Laplacian uses; directed != 0 adds the 1/sqrt(2).
+ * gsp_incidence_count / gsp_incidence_fill_*: D = Dt.T as CSR (the reference's D.tocsr()), each
+ *     row in increasing edge id, without a sort; t_indptr / t_indices / t_data is W^T as sorted
+ *     CSR for a directed graph, NULL for an undirected one; eptr as above (W's indptr if
+ *     directed).
+ * grad and div are gsp_spmm_* on Dt and D (difference.py:244, 331).
+ */
+int gsp_edge_offsets(int64_t n, const int32_t* indptr, const int32_t* indices, int32_t* eptr,
+                     void* stream);
+int gsp_incidence_count(int64_t n, const int32_t* indptr, const int32_t* indices,
+                        const int32_t* t_indptr, const int32_t* t_indices, int32_t* d_indptr,
+                        void* stream);
+
+#define GSPB200_DECLARE_DIFF_API(SUF, T)                                                         \
+  int gsp_edge_list_##SUF(int64_t n, int64_t n_edges, const int32_t* indptr,                     \
+                          const int32_t* indices, const T* data, const int32_t* eptr,            \
+                          int32_t* sources, int32_t* targets, T* weights, int32_t* dt_indptr,    \
+                          void* stream);                                                         \
+  int gsp_incidence_t_fill_##SUF(int64_t n_edges, const int32_t* sources,                        \
+                                 const int32_t* targets, const T* weights, const double* dw,     \
+                                 int lap_type, int directed, const int32_t* dt_indptr,           \
+                                 int32_t* dt_indices, T* dt_data, void* stream);                 \
+  int gsp_incidence_fill_##SUF(int64_t n, int lap_type, const int32_t* indptr,                   \
+                               const int32_t* indices, const T* data, const int32_t* eptr,       \
+                               const int32_t* t_indptr, const int32_t* t_indices,                \
+                               const T* t_data, const double* dw, const int32_t* d_indptr,       \
+                               int32_t* d_indices, T* d_data, void* stream);
+
+GSPB200_DECLARE_DIFF_API(f32, float)
+GSPB200_DECLARE_DIFF_API(f64, double)
 
 #ifdef __cplusplus
 }

@@ -90,10 +90,13 @@ cheby_step_rowgroup(int64_t row_begin, int64_t row_end,
 #pragma unroll
     for (int v = 0; v < VEC; ++v) acc.v[v] = xo.v[v] = xc.v[v] = T(0);
 
-    // streaming operands first: they are in flight while the gather runs
+    // streaming operands first: they are in flight while the gather runs.  x_cur's own row is
+    // read only when a term uses it, so a plain product (FIRST, beta = 0, no accumulator)
+    // indexes x_cur by column alone and the matrix may be rectangular (gsp_spmm_*)
     if (active) {
       if (!FIRST) xo = load_vec_stream<T, VEC>(x_old + row * nsig + c0);
-      xc = load_vec_ro<T, VEC>(x_cur + row * nsig + c0);
+      if (!FIRST || coef.beta != T(0) || nscales > 0)
+        xc = load_vec_ro<T, VEC>(x_cur + row * nsig + c0);
     }
 
     if (SPMM) {

@@ -65,6 +65,9 @@ int cheby_step(bool first, int64_t rb, int64_t re, const int32_t* indptr, const 
                double beta, double gamma, cudaStream_t st, bool add_source = false,
                const int64_t* out_perm = nullptr);   // x_new row of local row i is out_perm[i]
 
+// indptr[1..n] (row sizes on entry) := their inclusive scan, indptr[0] = 0 -- csrc/graph.cu
+int scan_rows(int32_t* indptr, int64_t n, cudaStream_t st);
+
 // dst[i,:] = src[idx[i],:] (scatter: dst[idx[i],:] = src[i,:]) -- csrc/graph.cu
 template <typename T>
 int move_rows(bool scatter, int64_t rows, const int64_t* idx, const T* src, int64_t width, T* dst,

@@ -43,7 +43,7 @@ __device__ __forceinline__ double warp_max(double v) {
 }
 
 // ---- inclusive scan of row sizes into indptr[1..n] -------------------------
-static int scan_rows(int32_t* indptr, int64_t n, cudaStream_t st) {
+int scan_rows(int32_t* indptr, int64_t n, cudaStream_t st) {
   // indptr[0] = 0 and indptr[1..n] hold row sizes on entry
   if (n == 0) return GSP_OK;
   size_t bytes = 0;

@@ -4,7 +4,8 @@ This is what ``Graph.W`` and ``Graph.L`` are in this engine (the reference
 holds ``scipy.sparse.csr_matrix`` objects, graph.py:109,620).  It offers the
 small read-only surface the filtering path and its callers use: ``shape``,
 ``nnz``, ``dot``, ``toarray``, ``diagonal``, plus ``to_scipy`` to leave the
-device.
+device.  The differential operator ``G.D`` is one too, (N, Ne), with its
+transpose attached as ``.T`` by the builder (graphs/difference.py).
 """
 import numpy as np
 
@@ -68,6 +69,16 @@ class DeviceCSR:
         return sparse.csr_matrix((self.data.cpu().numpy(), self.indices.cpu().numpy(),
                                   self.indptr.cpu().numpy()), shape=self.shape)
 
+    def to_scipy_csc(self):
+        """The matrix as ``scipy.sparse.csc_matrix``, for a matrix whose builder set ``.T``
+        (the differential operator: its CSC arrays are the CSR arrays of its transpose)."""
+        from scipy import sparse
+        T = getattr(self, "T", None)
+        if T is None:
+            raise AttributeError("to_scipy_csc needs the transpose built with the matrix (.T)")
+        return sparse.csc_matrix((T.data.cpu().numpy(), T.indices.cpu().numpy(),
+                                  T.indptr.cpu().numpy()), shape=self.shape)
+
     def toarray(self):
         return self.to_scipy().toarray()
 
@@ -76,16 +87,25 @@ class DeviceCSR:
 
     # -- product: scipy's csr_matrix.dot on the device SpMM kernel ------------------
     def dot(self, x):
-        """``A @ x`` for a vector or an (n, nsig) block; numpy in -> numpy out."""
+        """``A @ x`` for a vector or an (n, nsig) block; numpy in -> numpy out.
+
+        A rectangular matrix (the differential operator) always takes the SpMM kernel, which
+        reads x at column indices only; the SpMV's window form assumes a square matrix.
+        """
         torch = nat.require_cuda()
         host = not torch.is_tensor(x)
         xt = torch.as_tensor(np.asarray(x) if host else x).to(device=self.device, dtype=self.dtype)
         if xt.shape[0] != self.shape[1]:
             raise ValueError("dimension mismatch")
-        flat = xt.reshape(xt.shape[0], -1).contiguous()
+        flat = xt.reshape(xt.shape[0], int(np.prod(xt.shape[1:]))).contiguous()
+        square = self.shape[0] == self.shape[1]
+        if not square and (flat.numel() == 0 or self.shape[0] == 0):
+            y = torch.zeros((self.shape[0], flat.shape[1]), dtype=self.dtype, device=self.device)
+            y = y.reshape((self.shape[0],) + tuple(xt.shape[1:]))
+            return y.cpu().numpy() if host else y
         y = torch.empty((self.shape[0], flat.shape[1]), dtype=self.dtype, device=self.device)
         with torch.cuda.device(self.device):
-            if flat.shape[1] == 1:                      # one vector: the sub-warp SpMV
+            if flat.shape[1] == 1 and square:          # one vector: the sub-warp SpMV
                 nat.call("gsp_spmv_" + nat.suffix(self.dtype), nat.i64(self.shape[0]),
                          nat.i64(self.nnz), self.indptr, self.indices, self.data, flat, y,
                          nat.stream_ptr(self.device))

@@ -3,12 +3,14 @@
 Mirror of the part of ``pygsp.graphs.Graph`` that the Chebyshev filtering path
 uses (pygsp/graphs/graph.py:98-176 constructor, :510-630 compute_laplacian,
 :632-640 _check_signal, :729-838 d / dw, :840-960 lmax / estimate_lmax /
-_get_upper_bound, :368-405 is_directed) and, through ``FourierMixIn``
-(graphs/fourier.py), of the Fourier basis.  Same constructor signature, same
-attributes, same exceptions and log messages; the adjacency, the Laplacian and
-every vector derived from them live on the GPU and are produced by the kernels
-of ``libgspb200`` (csrc/graph.cu, csrc/lanczos.cu).  Out of scope here, as in
-SURVEY.md section 2: differential operator, plotting, IO.
+_get_upper_bound, :368-405 is_directed), through ``FourierMixIn``
+(graphs/fourier.py) of the Fourier basis, and through ``DifferenceMixIn``
+(graphs/difference.py) of the differential operator, ``get_edge_list`` and
+``dirichlet_energy``.  Same constructor signature, same attributes, same
+exceptions and log messages; the adjacency, the Laplacian and every vector
+derived from them live on the GPU and are produced by the kernels of
+``libgspb200`` (csrc/graph.cu, csrc/lanczos.cu, csrc/difference.cu).  Out of
+scope here, as in SURVEY.md section 2: plotting, IO.
 """
 import numpy as np
 from scipy import sparse
@@ -16,12 +18,13 @@ from scipy import sparse
 from .. import _native as nat
 from .. import utils
 from .csr import DeviceCSR
+from .difference import DifferenceMixIn
 from .fourier import FourierMixIn
 
 _LAP = {"combinatorial": 0, "normalized": 1}
 
 
-class Graph(FourierMixIn):
+class Graph(FourierMixIn, DifferenceMixIn):
     r"""Graph defined by a (weighted) adjacency matrix.
 
     Parameters
@@ -113,6 +116,7 @@ class Graph(FourierMixIn):
         self._lmax_method = None
         self._lanczos_steps = None
         self._clear_fourier_basis()
+        self._D = None
 
         self.lap_type = lap_type
         self.compute_laplacian(lap_type)
@@ -281,10 +285,12 @@ class Graph(FourierMixIn):
         if lap_type != self.lap_type:
             # the reference forgets _lmax_method here, so that G.lmax then returns
             # None (SURVEY.md 3.5); both are reset in this implementation.  The Fourier
-            # basis of the old Laplacian goes too (graph.py:605-608).
+            # basis and the differential operator of the old Laplacian go too
+            # (graph.py:605-609).
             self._lmax = None
             self._lmax_method = None
             self._clear_fourier_basis()
+            self._D = None
         self.lap_type = lap_type
 
         torch = nat.require_cuda()
