@@ -460,6 +460,64 @@ int gsp_incidence_count(int64_t n, const int32_t* indptr, const int32_t* indices
 GSPB200_DECLARE_DIFF_API(f32, float)
 GSPB200_DECLARE_DIFF_API(f64, double)
 
+/* ------------------------------------------------------------------ connectivity ---
+ * pygsp/graphs/graph.py:192-366, 444-508 on a canonical CSR adjacency W (n x n).  Vertex ids,
+ * labels and positions are int32; counters are int64.
+ * gsp_cc_labels_*:     the BFS of is_connected (graph.py:343-363, undirected) and of
+ *     extract_components (:483-500).  labels[v] = smallest vertex id of v's connected component
+ *     (union-find, deterministic).  W must have a symmetric structure; an edge is every stored
+ *     entry, or only the entries with weight > 0 when positive_only != 0 (A = W > 0 of
+ *     extract_components).  n_components (may be NULL) receives the number of components.
+ * gsp_reach_init / gsp_reach_levels: the BFS of is_connected for a directed graph (:343-363),
+ *     through W and again through W^T.  visited (n), queue (2 n) and state (4 int64) belong to
+ *     the caller.  init marks `source`; each levels call runs BFS levels
+ *     [level0, level0 + n_levels) (one launch per level, nothing synchronises).  After levels
+ *     [0, L) the search is over when state[L % 3] == 0; state[3] then counts the vertices
+ *     reached.
+ * gsp_vertex_map:      multiplicity map of a vertex list v (m entries in [0, n), repeats
+ *     allowed) -- the row / column selection of W[vertices, :][:, vertices] (:247).
+ *     mpos[mptr[u] .. mptr[u + 1]) are the positions p with v[p] == u, increasing; mptr has
+ *     n + 1 entries, mpos m.
+ * gsp_subgraph_count / gsp_subgraph_fill_*: W[v, :][:, v] (:247) as CSR (m x m).  labels (may be
+ *     NULL) keeps an entry (u, c) only when labels[u] == labels[c].  count writes s_indptr
+ *     (m + 1) and the number of entries to *nnz (device); s_indptr is meaningful only when
+ *     *nnz < 2^31, which the caller checks before allocating.  fill writes the entries, each row
+ *     in W's column order mapped through mpos: sorted when v is strictly increasing, and
+ *     block-diagonal sorted when v lists the vertices by (label, id) and labels is given.
+ *     Otherwise the caller sorts the rows (s_rows, may be NULL, receives each entry's row for
+ *     gsp_coo_to_csr_*); no two entries coincide.
+ * gsp_component_order: the vertices sorted by (label, id) into perm (n); comp_ptr (n + 1) gets
+ *     the first position of each component in that order, in increasing order of smallest
+ *     vertex, and n at index *n_components (device, may be NULL).
+ * gsp_weights_not_one_*: is_weighted (:292), not all(W.data == 1): *flag = 1 if an entry differs
+ *     from 1, else 0.
+ */
+int gsp_reach_init(int64_t n, int32_t source, int32_t* visited, int32_t* queue, int64_t* state,
+                   void* stream);
+int gsp_reach_levels(int64_t n, const int32_t* indptr, const int32_t* indices, int32_t* visited,
+                     int32_t* queue, int64_t* state, int64_t level0, int n_levels, void* stream);
+int gsp_vertex_map(int64_t n, int64_t m, const int32_t* v, int32_t* mptr, int32_t* mpos,
+                   void* stream);
+int gsp_subgraph_count(int64_t m, const int32_t* indptr, const int32_t* indices, const int32_t* v,
+                       const int32_t* mptr, const int32_t* labels, int32_t* s_indptr,
+                       int64_t* nnz, void* stream);
+int gsp_component_order(int64_t n, const int32_t* labels, int32_t* perm, int32_t* comp_ptr,
+                        int64_t* n_components, void* stream);
+
+#define GSPB200_DECLARE_CONN_API(SUF, T)                                                         \
+  int gsp_cc_labels_##SUF(int64_t n, const int32_t* indptr, const int32_t* indices,              \
+                          const T* data, int positive_only, int32_t* labels,                     \
+                          int64_t* n_components, void* stream);                                  \
+  int gsp_subgraph_fill_##SUF(int64_t m, const int32_t* indptr, const int32_t* indices,          \
+                              const T* data, const int32_t* v, const int32_t* mptr,              \
+                              const int32_t* mpos, const int32_t* labels,                        \
+                              const int32_t* s_indptr, int32_t* s_indices, T* s_data,            \
+                              int32_t* s_rows, void* stream);                                    \
+  int gsp_weights_not_one_##SUF(int64_t nnz, const T* data, int32_t* flag, void* stream);
+
+GSPB200_DECLARE_CONN_API(f32, float)
+GSPB200_DECLARE_CONN_API(f64, double)
+
 #ifdef __cplusplus
 }
 #endif

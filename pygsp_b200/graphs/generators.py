@@ -495,6 +495,12 @@ def sbm_adjacency(N=1024, k=5, z=None, p=0.7, q=None, seed=None):
     (tests/test_generators_cpu.py).
     """
     rng = np.random.default_rng(seed)
+    z, M = _sbm_blocks(rng, N, k, z, p, q)
+    return _sbm_draw(rng, N, k, z, M), z
+
+
+def _sbm_blocks(rng, N, k, z, p, q):
+    """Block assignment z (drawn from rng when None) and the k x k probability matrix M."""
     if z is None:
         z = np.sort(rng.integers(0, k, N))
     z = np.asarray(z)
@@ -513,6 +519,11 @@ def sbm_adjacency(N=1024, k=5, z=None, p=0.7, q=None, seed=None):
         raise ValueError("Probabilities should be in [0, 1].")
     if np.any(np.diff(z) < 0):
         raise ValueError("z must be sorted (blocks contiguous) for the vectorised sampler")
+    return z, M
+
+
+def _sbm_draw(rng, N, k, z, M):
+    """One draw of the SBM adjacency (canonical CSR) for blocks z and probabilities M."""
     start = np.searchsorted(z, np.arange(k), side="left")
     size = np.searchsorted(z, np.arange(k), side="right") - start
 
@@ -554,15 +565,37 @@ def sbm_adjacency(N=1024, k=5, z=None, p=0.7, q=None, seed=None):
     W = sparse.coo_matrix((np.ones(2 * r.size), (np.concatenate([r, c]), np.concatenate([c, r]))),
                           shape=(N, N)).tocsr()
     W.sort_indices()
-    return W, z
+    return W
 
 
 class StochasticBlockModel(Graph):
-    r"""Stochastic block model graph (undirected, no self-loops); see :func:`sbm_adjacency`."""
+    r"""Stochastic block model graph (undirected, no self-loops); see :func:`sbm_adjacency`.
 
-    def __init__(self, N=1024, k=5, z=None, p=0.7, q=None, seed=None, **kwargs):
+    ``connected=True`` draws z once and then resamples W from the same generator until the
+    graph is connected, at most ``n_try`` times (None: forever), as
+    stochasticblockmodel.py:125-157 does; it raises the reference's ``ValueError`` after
+    ``n_try`` failures.  With ``connected=False`` the graph is :func:`sbm_adjacency`'s.
+    """
+
+    def __init__(self, N=1024, k=5, z=None, p=0.7, q=None, seed=None, connected=False,
+                 n_try=10, **kwargs):
         self.k, self.p, self.q, self.seed = k, p, q, seed
-        W, self.z = sbm_adjacency(N, k, z, p, q, seed)
+        self.connected, self.n_try = connected, n_try
+        rng = np.random.default_rng(seed)
+        self.z, M = _sbm_blocks(rng, N, k, z, p, q)
+        W = None
+        while n_try is None or n_try > 0:
+            W = _sbm_draw(rng, N, k, self.z, M)
+            if not connected or Graph(W, dtype=kwargs.get("dtype"),
+                                      device=kwargs.get("device")).is_connected():
+                break
+            if n_try is not None:
+                n_try -= 1
+        if connected and n_try == 0:
+            raise ValueError("The graph could not be connected after {} trials. Increase the "
+                             "connection probability or the number of trials.".format(self.n_try))
+        if W is None:
+            W = _sbm_draw(rng, N, k, self.z, M)
         self.info = {"node_com": self.z, "comm_sizes": np.bincount(self.z, minlength=k),
                      "world_rad": np.sqrt(N)}
         super().__init__(W, **kwargs)

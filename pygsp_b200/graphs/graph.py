@@ -4,12 +4,15 @@ Mirror of the part of ``pygsp.graphs.Graph`` that the Chebyshev filtering path
 uses (pygsp/graphs/graph.py:98-176 constructor, :510-630 compute_laplacian,
 :632-640 _check_signal, :729-838 d / dw, :840-960 lmax / estimate_lmax /
 _get_upper_bound, :368-405 is_directed), through ``FourierMixIn``
-(graphs/fourier.py) of the Fourier basis, and through ``DifferenceMixIn``
+(graphs/fourier.py) of the Fourier basis, through ``DifferenceMixIn``
 (graphs/difference.py) of the differential operator, ``get_edge_list`` and
-``dirichlet_energy``.  Same constructor signature, same attributes, same
+``dirichlet_energy``, and through ``ConnectivityMixIn`` (graphs/connectivity.py) of
+``is_connected``, ``extract_components``, ``subgraph``, ``set_signal`` and
+``is_weighted``.  Same constructor signature, same attributes, same
 exceptions and log messages; the adjacency, the Laplacian and every vector
 derived from them live on the GPU and are produced by the kernels of
-``libgspb200`` (csrc/graph.cu, csrc/lanczos.cu, csrc/difference.cu).  Out of
+``libgspb200`` (csrc/graph.cu, csrc/lanczos.cu, csrc/difference.cu,
+csrc/connectivity.cu).  Out of
 scope here, as in SURVEY.md section 2: plotting, IO.
 """
 import numpy as np
@@ -17,6 +20,7 @@ from scipy import sparse
 
 from .. import _native as nat
 from .. import utils
+from .connectivity import ConnectivityMixIn
 from .csr import DeviceCSR
 from .difference import DifferenceMixIn
 from .fourier import FourierMixIn
@@ -24,7 +28,7 @@ from .fourier import FourierMixIn
 _LAP = {"combinatorial": 0, "normalized": 1}
 
 
-class Graph(FourierMixIn, DifferenceMixIn):
+class Graph(FourierMixIn, DifferenceMixIn, ConnectivityMixIn):
     r"""Graph defined by a (weighted) adjacency matrix.
 
     Parameters
