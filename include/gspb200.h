@@ -241,6 +241,35 @@ GSPB200_DECLARE_CG_API(f64, double)
 GSPB200_DECLARE_BLOCK_API(f32, float)
 GSPB200_DECLARE_BLOCK_API(f64, double)
 
+/* ------------------------------------------------------- Lanczos filtering ---
+ * Per-signal Krylov bases of pygsp/filters/approximations.py:228-341 (lanczos_op, lanczos):
+ * one independent Lanczos process per column of a row-major (n, nsig) block, with full
+ * reorthogonalisation against that column's own basis.  Columns never mix, and every sum over
+ * rows accumulates in double over a row partition that depends on n only, so a column's bits do
+ * not depend on nsig or on the other columns.  Scratch is stream-ordered (cudaMallocAsync).
+ * gsp_krylov_basis_*: A is n x ncols CSR and must be square (ncols != n is refused before any
+ *   launch: the SpMM reads the basis at A's column indices).  V is (order + 1, n, nsig)
+ *   (vector k of column j is V[k, :, j]; slot order is workspace).  On return, for every column j (arrays of double, row-major, on the device):
+ *   alpha (order x nsig) the diagonal of T_j, beta (order x nsig) its off-diagonal
+ *   (beta[k] = beta_k couples vectors k - 1 and k; beta[0] = ||x_j||), vs (order x nsig) = V^T x
+ *   and m (nsig, int32) the Krylov dimension.  A column stops growing (breakdown) when
+ *   beta_{k+1} <= 16 eps max(largest |alpha|, |beta| so far, ||A||_inf); its vectors past m and
+ *   its alpha, beta past the leading m x m block are zero.  A zero column has m = 0.
+ * gsp_krylov_combine_*: Y[f, r, j] = sum_{i < k} V[i, r, j] W[f, i, j] for W (nf, k, nsig)
+ *   double; Y is (nf, n, ldy) with ldy >= nsig (a column range of a wider block).  One pass
+ *   over V for up to 16 filters.
+ */
+#define GSPB200_DECLARE_KRYLOV_API(SUF, T)                                                       \
+  int gsp_krylov_basis_##SUF(int64_t n, int64_t ncols, const int32_t* indptr,                   \
+                             const int32_t* indices,                                             \
+                             const T* data, const T* x, int64_t nsig, int order, T* V,           \
+                             double* alpha, double* beta, double* vs, int32_t* m, void* stream); \
+  int gsp_krylov_combine_##SUF(int64_t n, const T* V, int64_t k, const double* W, int64_t nf,   \
+                               int64_t nsig, T* Y, int64_t ldy, void* stream);
+
+GSPB200_DECLARE_KRYLOV_API(f32, float)
+GSPB200_DECLARE_KRYLOV_API(f64, double)
+
 /* ------------------------------------------------- host <-> device staging ---
  * Filter.filter() takes and returns host arrays (filter.py:146-328).  To overlap the PCIe
  * transfers with the recurrence the signal block is processed in COLUMN chunks; a chunk of a

@@ -241,3 +241,185 @@ def compute_jackson_cheby_coeff(filter_bounds, delta_lambda, m):
     t = np.pi / (m + 2)
     damp = ((1 - j / (m + 2)) * np.sin(t) * np.cos(j * t) + np.cos(t) * np.sin(j * t) / (m + 2)) / np.sin(t)
     return ch, ch * damp
+
+
+# ------------------------------------------------------------------------------ Lanczos
+def _check_square(shape):
+    """Lanczos needs a square matrix: its products are read back as basis vectors."""
+    if len(shape) != 2 or shape[0] != shape[1]:
+        raise ValueError("The matrix must be square, got shape {}.".format(tuple(shape)))
+
+
+def _krylov_basis(L, x, order):
+    """One Lanczos process per column of the device block x (N, nsig), csrc/krylov.cu.
+
+    Returns the device basis (order + 1, N, nsig) (slot ``order`` is workspace) and, on the
+    host, alpha and beta (order, nsig), V^T x (order, nsig) and the Krylov dimensions m (nsig,):
+    the only transfer, O(order * nsig) numbers."""
+    torch = nat.require_cuda()
+    n, nsig = x.shape
+    _check_square(L.shape)
+    V = torch.empty((order + 1, n, nsig), dtype=L.dtype, device=L.device)
+    small = torch.empty((3, order, nsig), dtype=torch.float64, device=L.device)
+    m = torch.empty(nsig, dtype=torch.int32, device=L.device)
+    with torch.cuda.device(L.device):
+        nat.call("gsp_krylov_basis_" + nat.suffix(L.dtype), nat.i64(n), nat.i64(L.shape[1]),
+                 L.indptr, L.indices, L.data, x, nat.i64(nsig), nat.i32(order), V, small[0], small[1], small[2], m,
+                 nat.stream_ptr(L.device))
+    small, m = small.cpu().numpy(), m.cpu().numpy()
+    return V, small[0], small[1], small[2], m
+
+
+def _tridiagonals(alpha, beta):
+    """T_j (order x order) of every column: (nsig, order, order)."""
+    order, nsig = alpha.shape
+    T = np.zeros((nsig, order, order))
+    i = np.arange(order)
+    T[:, i, i] = alpha.T
+    T[:, i[1:], i[:-1]] = T[:, i[:-1], i[1:]] = beta[1:].T
+    return T
+
+
+def _lanczos_coefficients(evaluate, alpha, beta, vs, m):
+    """W (Nf, order, nsig): column j's combination Q_j f(max(Theta_j, 0)) Q_j^T (V_j^T s_j)
+    over its leading m_j x m_j block, zero past it.  Host float64 ``eigh``, batched over the
+    columns of one Krylov dimension."""
+    order, nsig = alpha.shape
+    T = _tridiagonals(alpha, beta)
+    W = None
+    for mj in np.unique(m[m > 0]):
+        cols = np.flatnonzero(m == mj)
+        e, Q = np.linalg.eigh(T[np.ix_(cols, np.arange(mj), np.arange(mj))])   # (c, m), (c, m, m)
+        e[e < 0] = 0
+        fe = np.asarray(evaluate(e), dtype=np.float64).reshape(-1, cols.size, mj)
+        if W is None:
+            W = np.zeros((fe.shape[0], order, nsig))
+        proj = np.einsum("cki,ck->ci", Q, vs[:mj, cols].T)
+        W[:, :mj, cols] = np.einsum("cik,fck->fic", Q, fe * proj[None])
+    if W is None:                                     # every column is zero
+        W = np.zeros((np.asarray(evaluate(np.zeros(1))).reshape(-1, 1).shape[0], order, nsig))
+    return W
+
+
+def lanczos_op_device(L, evaluate, x, order, max_columns=None):
+    """Device-to-device core of :func:`lanczos_op`: x (N, nsig) tensor -> (Nf, N, nsig) tensor.
+
+    The basis takes (order + 1) N nsig elements.  When that does not fit in the device memory
+    left once the output is allocated (or ``max_columns`` is given) the columns are processed in
+    chunks; the results are the same bits, since no sum mixes columns or depends on their
+    number."""
+    torch = nat.require_cuda()
+    n, nsig = x.shape
+    nf = np.asarray(evaluate(np.zeros(1))).reshape(-1, 1).shape[0]
+    out = torch.empty((nf, n, nsig), dtype=L.dtype, device=L.device)
+    if nsig == 0:
+        return out
+    item = x.element_size()
+    # basis, the column's copy of the signal when chunked, reduction partials, W
+    per_column = (order + 2) * n * item + 264 * order * 8 + nf * order * 8
+    if max_columns is None:
+        free, _ = torch.cuda.mem_get_info(L.device)
+        free += torch.cuda.memory_reserved(L.device) - torch.cuda.memory_allocated(L.device)
+        max_columns = int(free * 0.9) // per_column
+        if max_columns < 1:
+            raise ValueError(
+                "The Lanczos basis of one signal ({0} vectors of {1} x {2} bytes, {3:.2f} GB) does "
+                "not fit in the free device memory ({4:.2f} GB). Lower the order.".format(
+                    order + 1, n, item, per_column / 2 ** 30, free / 2 ** 30))
+    step = max(1, min(int(max_columns), nsig))
+    for j0 in range(0, nsig, step):
+        j1 = min(nsig, j0 + step)
+        xc = x if (j0, j1) == (0, nsig) else x[:, j0:j1].contiguous()
+        V, alpha, beta, vs, m = _krylov_basis(L, xc, order)
+        W = _lanczos_coefficients(evaluate, alpha, beta, vs, m)
+        Wd = torch.as_tensor(W, device=L.device).contiguous()
+        with torch.cuda.device(L.device):
+            nat.call("gsp_krylov_combine_" + nat.suffix(L.dtype), nat.i64(n), V, nat.i64(order),
+                     Wd, nat.i64(nf), nat.i64(j1 - j0), out[:, :, j0:], nat.i64(nsig),
+                     nat.stream_ptr(L.device))
+        del V
+    return out
+
+
+def lanczos_op(f, s, order=30):
+    r"""Lanczos approximation of the filter bank ``f`` applied to ``s``.
+
+    Same contract as the reference (approximations.py:228-278): ``s`` (N,) gives (Nf*N,), ``s``
+    (N, Nv) gives (Nf*N, Nv), with filter-major row blocks as in :func:`cheby_op`.  Column j is
+    ``V_j Q_j f(max(Theta_j, 0)) Q_j^T (V_j^T s_j)`` where ``V_j`` is the order-``order`` Krylov
+    basis of L and s_j (full reorthogonalisation) and ``Q_j Theta_j Q_j^T`` the eigendecomposition
+    of its tridiagonal ``T_j``.  Each column has its own process on the device (csrc/krylov.cu);
+    the ``eigh`` of the small ``T_j`` runs on the host in float64.  A column whose Krylov space
+    becomes invariant stops growing (the result is then exact) and a zero column gives zeros; the
+    reference fails on both.  Input and output kinds and the arithmetic type follow
+    :func:`cheby_op`.
+    """
+    order = int(order)
+    if order < 1:
+        raise ValueError("The order must be at least 1, got {}.".format(order))
+    G = f.G
+    L = _laplacian_on_device(G)
+    x, one_d, kind = _as_device_block(_GraphView(L), s)
+    if x.shape[0] != G.N:
+        raise ValueError("First dimension must be the number of vertices "
+                         "G.N = {}, got {}.".format(G.N, tuple(x.shape)))
+    r = lanczos_op_device(L, f.evaluate, x, order)
+    r = r.reshape(r.shape[0] * G.N, x.shape[1])
+    if one_d:
+        r = r.reshape(-1)
+    out = _leave_device(r, kind)
+    if kind == "numpy" and not isinstance(G.L, type(L)):
+        out = out.astype(np.float64, copy=False)     # a reference graph expects float64 back
+    return out
+
+
+def _orth_from_gram(C, M, order, m):
+    """The reference's ``||V^T V - M||_F`` after each step (approximations.py:314, 337) from the
+    Gram C of the final basis: vector i of signal j is in place after step k when
+    i <= min(k, m_j - 1), and a vector not yet in place is zero, so each of its entries of
+    V^T V - M is -M."""
+    total = M * order
+    orth = np.zeros(order)
+    for k in range(order):
+        idx = np.concatenate([j * order + np.arange(min(k + 1, int(m[j]))) for j in range(M)])
+        sub = C[np.ix_(idx, idx)] - M
+        orth[k] = np.sqrt(np.sum(sub ** 2) + (total ** 2 - idx.size ** 2) * float(M) ** 2)
+    return orth
+
+
+def lanczos(A, order, x):
+    r"""Lanczos bases of ``A`` for the columns of ``x`` (approximations.py:281-341).
+
+    ``A`` is a :class:`~pygsp_b200.graphs.csr.DeviceCSR` or a SciPy sparse / dense NumPy matrix
+    (uploaded as float64 CSR); ``x`` is (N,) or (N, M).  Returns ``(V, H, orth)`` in the
+    reference's layout: V (N, M*order) with signal j's k-th vector in column ``j*order + k``, in
+    the kind of ``x``; H (order, M*order) with signal j's tridiagonal T_j in columns
+    ``j*order .. j*order + order - 1``; orth[k] = ``||V^T V - M||_F`` over the basis as it
+    stands after step k.  The M processes are independent (the reference couples them and
+    returns the first signal's T only; for M = 1 the two agree).  A signal whose Krylov space
+    becomes invariant after m < order steps keeps zero vectors and a zero T past m.
+    """
+    from scipy import sparse
+    from ..graphs.csr import DeviceCSR
+    from ..graphs.fourier import block_gram
+    order = int(order)
+    if order < 1:
+        raise ValueError("The order must be at least 1, got {}.".format(order))
+    _check_square(A.shape if hasattr(A, "shape") else np.shape(A))
+    torch = nat.require_cuda()
+    if not isinstance(A, DeviceCSR):
+        dev = torch.device("cuda:%d" % torch.cuda.current_device())
+        A = DeviceCSR.from_scipy(sparse.csr_matrix(A), torch.float64, dev)
+    x, _, kind = _as_device_block(_GraphView(A), x)
+    n, M = x.shape
+    if n != A.shape[0]:
+        raise ValueError("x has {} rows, A is {} x {}.".format(n, *A.shape))
+    if M == 0:
+        return _leave_device(x[:, :0], kind), np.zeros((order, 0)), np.zeros(order)
+    Vb, alpha, beta, _, m = _krylov_basis(A, x, order)
+    V = Vb[:order].permute(1, 2, 0).reshape(n, M * order).contiguous()
+    del Vb
+    C = block_gram(V, V).cpu().numpy()
+    T = _tridiagonals(alpha, beta)
+    H = np.concatenate(list(T), axis=1)
+    return _leave_device(V, kind), H, _orth_from_gram(C, M, order, m)
