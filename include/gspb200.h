@@ -67,7 +67,9 @@ int gsp_device_info(int* sm_count, int* cc_major, int* cc_minor, int64_t* l2_byt
 typedef struct gsp_tile_plan {
   int rows_per_tile;   /* rows of L per shared-memory stage */
   int slab_capacity;   /* CSR entries a stage can hold (>= the matrix's largest tile) */
-  int stages;          /* depth of the TMA ring */
+  int stages;          /* depth of the TMA ring of steps that stage vector tiles (a step whose
+                          stage holds only the CSR slab -- the first step, or x_old / r read
+                          directly as in the Clenshaw form -- runs a one-stage ring) */
   int consumer_warps;  /* warps that compute (one more warp produces); the two-packet lane
                           mapping of the Clenshaw form runs min(consumer_warps, 8) of them */
   int gather_unroll;   /* reserved (always 4: one LDS.128 group of CSR entries) */
