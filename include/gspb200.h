@@ -272,6 +272,44 @@ GSPB200_DECLARE_BLOCK_API(f64, double)
 GSPB200_DECLARE_KRYLOV_API(f32, float)
 GSPB200_DECLARE_KRYLOV_API(f64, double)
 
+/* ---------------------------------------------------------------- features ---
+ * pygsp/features.py without the frame (pygsp_b200/features.py).  The squared row norms of the
+ * frame, ||p(L) e_i||^2 for p = c0/2 T_0 + sum_k c_k T_k(Lt), Lt = 2 L / lmax - I, are
+ * sum_n d_n mu_n(i) with mu_n(i) = (T_n(Lt))_ii and d the Chebyshev series of p^2; one
+ * recurrence over identity probe blocks gives mu for every kernel.  The blocks T_k are produced
+ * by gsp_cheby_step_* (nscales = 0; first step alpha = 2/lmax, beta = -1; then alpha = 4/lmax,
+ * beta = -2, gamma = -1).
+ * gsp_probe_block_*: X (n, b) row-major = columns v0 .. v0 + b - 1 of the identity -- the
+ *   s = np.identity(N) that compute_frame filters (pygsp/filters/filter.py:599), b columns at a
+ *   time.
+ * gsp_cheby_moments_step_*: after step k (t_next = T_{k+1}, t_cur = T_k, both (n, b)), writes
+ *   sums[k][0][j] = sum_r t_next[r, j]^2 and sums[k][1][j] = sum_r t_next[r, j] t_cur[r, j] into
+ *   sums (m, 2, b) double.  Sums accumulate in double over a row partition that depends on n
+ *   only, so column j's sums do not depend on b or on the other columns.
+ * gsp_cheby_moments_finish: mu rows v0 .. v0 + b - 1 of mu (n, 2m + 1) double from sums after
+ *   the m steps: mu_0 = 1, mu_1 = sums[0][1], mu_{2k} = 2 sums[k-1][0] - 1,
+ *   mu_{2k+1} = 2 sums[k][1] - mu_1.  Stands for np.linalg.norm(tig, axis=1) of
+ *   compute_norm_tig (pygsp/features.py:58-59), with the atom combination done by
+ *   gsp_block_combine_f64.
+ * gsp_two_hop_count_*: np.dot(G.A, G.A) with G.A = W > 0 (pygsp/features.py:23,
+ *   graph.py:718-727), a boolean product: two_hop[i] = number of distinct c with W[i, k] > 0 and
+ *   W[k, c] > 0 for some k; degree[i] = number of k with W[i, k] > 0 (np.sum(G.A, axis=1)).
+ *   Exact for any degree distribution; scratch is bounded (heavy rows are processed in chunks).
+ *   The call synchronises `stream` (once, and once per chunk of heavy rows).
+ */
+#define GSPB200_DECLARE_MOMENTS_API(SUF, T)                                                      \
+  int gsp_probe_block_##SUF(int64_t n, int64_t v0, int64_t b, T* X, void* stream);              \
+  int gsp_cheby_moments_step_##SUF(int64_t n, const T* t_next, const T* t_cur, int64_t b, int m, \
+                                   int k, double* sums, void* stream);                           \
+  int gsp_two_hop_count_##SUF(int64_t n, const int32_t* indptr, const int32_t* indices,         \
+                              const T* data, int32_t* two_hop, int32_t* degree, void* stream);
+
+GSPB200_DECLARE_MOMENTS_API(f32, float)
+GSPB200_DECLARE_MOMENTS_API(f64, double)
+
+int gsp_cheby_moments_finish(int64_t n, int m, int64_t v0, int64_t b, const double* sums,
+                             double* mu, void* stream);
+
 /* ------------------------------------------------- host <-> device staging ---
  * Filter.filter() takes and returns host arrays (filter.py:146-328).  To overlap the PCIe
  * transfers with the recurrence the signal block is processed in COLUMN chunks; a chunk of a

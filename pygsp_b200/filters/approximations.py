@@ -243,6 +243,99 @@ def compute_jackson_cheby_coeff(filter_bounds, delta_lambda, m):
     return ch, ch * damp
 
 
+# ------------------------------------------------------------------- diagonal moments
+def cheby_square_coeff(c):
+    r"""Chebyshev series of ``p^2`` for ``p = c[0]/2 T_0 + sum_k c[k] T_k`` (the reference's
+    convention, approximations.py:99-112), in the same convention: ``p^2 = d[0]/2 T_0 +
+    sum_n d[n] T_n``, ``n <= 2 (len(c) - 1)``.  From ``T_j T_k = (T_{j+k} + T_{|j-k|}) / 2``.
+    ``c`` (m + 1,) gives (2m + 1,); an (Nf, m + 1) array gives (Nf, 2m + 1).  Host, float64."""
+    c = np.asarray(c, dtype=np.float64)
+    one = c.ndim == 1
+    c = np.atleast_2d(c)
+    nf, K = c.shape
+    a = c.copy()
+    a[:, 0] *= 0.5                                  # plain coefficients of T_0 .. T_m
+    e = np.zeros((nf, 2 * K - 1))
+    for j in range(K):
+        # a_j a_k / 2 goes to T_{j+k} and to T_{|j-k|}
+        e[:, j:j + K] += 0.5 * a[:, j:j + 1] * a
+        diff = np.abs(j - np.arange(K))
+        np.add.at(e, (slice(None), diff), 0.5 * a[:, j:j + 1] * a)
+    e[:, 0] *= 2.0                                  # back to the c0/2 convention
+    return e[0] if one else e
+
+
+def cheby_moments_device(L, lmax, order, width=None):
+    r"""Diagonal Chebyshev moments ``mu[i, n] = (T_n(Lt))_ii``, ``Lt = 2 L / lmax - I``,
+    n = 0 .. 2 order: a device (N, 2 order + 1) float64 tensor.
+
+    For every probe block of ``width`` identity columns (csrc/moments.cu), ``order`` steps of
+    the Chebyshev recurrence (``gsp_cheby_step_*`` with no accumulator: the tiled kernel at
+    float32 widths 8-128) give T_1 .. T_order of the block, and after each step one pass sums
+    ``||T_{k+1} e_i||^2`` and ``<T_{k+1} e_i, T_k e_i>`` in float64; ``mu_{2k} = 2 ||T_k e_i||^2 - 1``
+    and ``mu_{2k+1} = 2 <T_{k+1} e_i, T_k e_i> - mu_1``.  Then ``||p(L) e_i||^2 = mu[i] . d`` with
+    d of :func:`cheby_square_coeff` (d[0] halved) for any p of degree <= order.  A vertex's row is
+    the same bits whatever the width or the block it falls in.  The default width is 128 columns
+    for float32 and 64 for float64; it is lowered when two (N, width) blocks do not fit in the
+    free device memory left once mu is allocated."""
+    torch = nat.require_cuda()
+    order = int(order)
+    if order < 1:
+        raise ValueError("The order must be at least 1, got {}.".format(order))
+    n = L.shape[0]
+    if L.shape[1] != n:
+        raise ValueError("The Laplacian must be square, got shape {}.".format(tuple(L.shape)))
+    dev, sfx = L.device, nat.suffix(L.dtype)
+    item = L.data.element_size()
+    if width is None:
+        width = 128 if L.dtype == torch.float32 else 64
+    width = max(1, min(int(width), n))
+    K = 2 * order + 1
+    free, _ = torch.cuda.mem_get_info(dev)
+    free += torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
+    mu_bytes = n * K * 8
+    # two probe blocks, the step sums and the reduction partials per column
+    per_column = 2 * n * item + order * 2 * 8 + 264 * 2 * 8
+    room = int(free * 0.9) - mu_bytes
+    if room < per_column:
+        raise ValueError(
+            "The moments (N = {0}, order {1}: {2:.2f} GB) and one probe column do not fit in the "
+            "free device memory ({3:.2f} GB). Lower the order.".format(
+                n, order, mu_bytes / 2 ** 30, free / 2 ** 30))
+    width = min(width, room // per_column)
+    mu = torch.empty((n, K), dtype=torch.float64, device=dev)
+    blocks = torch.empty((2, n, width), dtype=L.dtype, device=dev)
+    sums = torch.empty((order, 2, width), dtype=torch.float64, device=dev)
+    zero = np.zeros(1)
+    stream = nat.stream_ptr(dev)
+    with torch.cuda.device(dev):
+        for v0 in range(0, n, width):
+            b = min(width, n - v0)
+            A = blocks[0].view(-1)[:n * b].view(n, b)       # T_{k-1}, then T_{k+1}
+            B = blocks[1].view(-1)[:n * b].view(n, b)       # T_k
+            plan = L.tile_plan(b, 0)
+            nat.call("gsp_probe_block_" + sfx, nat.i64(n), nat.i64(v0), nat.i64(b), A, stream)
+            # T_1 = (2 / lmax) L T_0 - T_0
+            nat.call("gsp_cheby_step_" + sfx, nat.i32(1), nat.i64(0), nat.i64(n), nat.i64(L.nnz),
+                     L.indptr, L.indices, L.data, A, A, B, B, nat.i64(n), nat.i64(b), nat.i32(0),
+                     zero, zero, nat.f64(2.0 / lmax), nat.f64(-1.0), nat.f64(0.0), plan, stream)
+            nat.call("gsp_cheby_moments_step_" + sfx, nat.i64(n), B, A, nat.i64(b),
+                     nat.i32(order), nat.i32(0), sums, stream)
+            cur, old = B, A
+            for k in range(1, order):
+                # T_{k+1} = (4 / lmax) L T_k - 2 T_k - T_{k-1}, written over T_{k-1} (row-local)
+                nat.call("gsp_cheby_step_" + sfx, nat.i32(0), nat.i64(0), nat.i64(n),
+                         nat.i64(L.nnz), L.indptr, L.indices, L.data, cur, old, old, old,
+                         nat.i64(n), nat.i64(b), nat.i32(0), zero, zero, nat.f64(4.0 / lmax),
+                         nat.f64(-2.0), nat.f64(-1.0), plan, stream)
+                nat.call("gsp_cheby_moments_step_" + sfx, nat.i64(n), old, cur, nat.i64(b),
+                         nat.i32(order), nat.i32(k), sums, stream)
+                cur, old = old, cur
+            nat.call("gsp_cheby_moments_finish", nat.i64(n), nat.i32(order), nat.i64(v0),
+                     nat.i64(b), sums, mu, stream)
+    return mu
+
+
 # ------------------------------------------------------------------------------ Lanczos
 def _check_square(shape):
     """Lanczos needs a square matrix: its products are read back as basis vectors."""
