@@ -587,6 +587,44 @@ int gsp_component_order(int64_t n, const int32_t* labels, int32_t* perm, int32_t
 GSPB200_DECLARE_CONN_API(f32, float)
 GSPB200_DECLARE_CONN_API(f64, double)
 
+/* ----------------------------------------------------------- multiresolution ---
+ * pygsp/reduction.py: Kron reduction, effective resistances and the edge sampler of
+ * graph_sparsify (pygsp_b200/reduction.py, csrc/schur.cu).  Kron reduction is always float64.
+ * The matrix M (n x n, canonical CSR) is split into kept and removed vertices by `slot`:
+ * slot[v] >= 0 for a removed vertex (its position in its component), slot[v] = -1 - (index of v
+ * among the kept vertices) for a kept one.  The removed vertices are listed component by
+ * component in cvert, component c at cvert[cptr[c] .. cptr[c + 1]); its kept neighbours B, in
+ * increasing kept index, at bidx[bptr[c] .. bptr[c + 1]).
+ * gsp_schur_small_f64: the blocks -M_BS M_SS^-1 M_SB of linalg.spsolve / dot at reduction.py:358,
+ *   one CTA per component listed in comps (n_small entries): Cholesky of M_SS in shared memory,
+ *   then |B|^2 COO triplets (row-major over B x B, kept indices) at rows / cols / vals +
+ *   out_off[c].  smem_bytes >= 8 (s^2 + s + s b) + 4 b for every listed component.  *status (device)
+ *   is set to 1 if some M_SS is not positive definite, else 0.
+ * gsp_schur_gather_f64: the dense blocks M_SS (s x s) into A and M_SB (s x nb) into B, both
+ *   row-major, of the component whose vertices are cvert[0 .. s) and whose kept neighbours are
+ *   bidx[0 .. nb) -- the input of a dense float64 Cholesky for a large component.
+ * gsp_edge_resistance_f64: R[e] = Ainv[u][u] + Ainv[v][v] - Ainv[u][v] - Ainv[v][u] for
+ *   u = erow[e], v = ecol[e] and a dense row-major Ainv (ld lda) -- the effective resistances
+ *   resistance_distances[start_nodes, end_nodes] of graph_sparsify (:84, :101).
+ * gsp_sparsify_sample: counts[e] (int64, ne) = how many of q draws from P(e) = weights[e] /
+ *   sum(weights) (uint64 integer weights, sum < 2^64) picked e -- dist.rvs(size=q) and the
+ *   removed stats.itemfreq of graph_sparsify (:104-115).  Draws come from Philox streams of
+ *   `seed` (curand_kernel.h): the counts depend on (seed, weights, q) only.
+ */
+int gsp_schur_small_f64(const int32_t* indptr, const int32_t* indices, const double* data,
+                        const int32_t* slot, const int32_t* cvert, const int32_t* cptr,
+                        const int32_t* bptr, const int32_t* bidx, int64_t n_small,
+                        const int32_t* comps, int smem_bytes, const int64_t* out_off,
+                        int32_t* rows, int32_t* cols, double* vals, int32_t* status,
+                        void* stream);
+int gsp_schur_gather_f64(const int32_t* indptr, const int32_t* indices, const double* data,
+                         const int32_t* slot, const int32_t* cvert, int64_t s,
+                         const int32_t* bidx, int64_t nb, double* A, double* B, void* stream);
+int gsp_edge_resistance_f64(int64_t ne, const int32_t* erow, const int32_t* ecol,
+                            const double* ainv, int64_t lda, double* R, void* stream);
+int gsp_sparsify_sample(int64_t ne, const uint64_t* weights, int64_t q, uint64_t seed,
+                        int64_t* counts, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

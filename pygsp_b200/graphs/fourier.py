@@ -219,6 +219,56 @@ class FourierMixIn:
         raise ValueError("The Chebyshev-filtered subspace iteration did not converge in {} "
                          "iterations.".format(cap))
 
+    def _largest_eigenvector(self, *, seed=0, max_iter=None):
+        """Eigenvector of the largest eigenvalue of L as a float64 host array (unit norm).
+
+        What graph_multiresolution down-samples with (reduction.py:271-275): the last column of a
+        full basis when there is one; a dense float64 ``eigh`` for small graphs; otherwise
+        Chebyshev-filtered subspace iteration on the reflected operator ``b_up I - L`` (its
+        smallest eigenpair is L's largest), through the same fused step with alpha and beta
+        transformed, from a start block that is a counter-based function of ``seed``.  Stops when
+        ``||L v - theta v|| <= tol b_up`` (tol 1e-10 in float64, 1e-5 in float32).
+        """
+        torch = nat.require_cuda()
+        n = self.n_vertices
+        if self._U is not None and len(self._e) == n:
+            return self._U[:, -1].double().cpu().numpy()
+        if n <= DENSE_CROSSOVER:
+            with torch.cuda.device(self.device):
+                _, U = torch.linalg.eigh(self._dense_laplacian())
+            return U[:, -1].cpu().numpy()
+        cap = MAX_ITERATIONS if max_iter is None else int(max_iter)
+        tol = 1e-10 if self.dtype == torch.float64 else 1e-5
+        b = block_width(1, n)
+        upper = float(self._get_upper_bound())
+        rng = _Seeds(seed)
+        X = block_random(n, b, rng.next(), self.dtype, self.device)
+        X = self._orthonormalize(X, rng)
+        X, LX, theta = self._rayleigh_ritz(X)
+        for _ in range(cap):
+            # spectrum of b_up I - L on the block: upper - theta; damp [a, upper] of it
+            a = min(upper - float(theta[0]), 0.95 * upper)
+            width = np.arccosh((upper + a) / (upper - a))
+            deg = int(max(2, min(FILTER_DEGREE, np.arccosh(_FILTER_RANGE[self._sfx]) // width)))
+            X = self._chebyshev_filter(X, deg, a, upper, reflect=True)
+            X = self._orthonormalize(X, rng)
+            X, LX, theta = self._rayleigh_ritz(X)
+            res = np.sqrt(max(float(block_residual(X, LX, theta)[-1]), 0.0))
+            if res <= tol * upper:
+                return X[:, -1].double().cpu().numpy()
+        raise ValueError("The Chebyshev-filtered subspace iteration for the largest eigenvector "
+                         "did not converge in {} iterations.".format(cap))
+
+    def _dense_laplacian(self):
+        """L as a dense float64 device matrix."""
+        torch = nat.require_cuda()
+        n, L = self.n_vertices, self.L
+        rows = torch.repeat_interleave(torch.arange(n, device=self.device),
+                                       (L.indptr[1:] - L.indptr[:-1]).long())
+        dense = torch.zeros((n, n), dtype=torch.float64, device=self.device)
+        dense[rows, L.indices.long()] = L.data.double()
+        return dense
+
     def _apply_laplacian(self, X):
         """L X by the recurrence step (alpha = 1, beta = 0): the tiled kernel where it applies."""
         torch = nat.require_cuda()
@@ -232,8 +282,10 @@ class FourierMixIn:
                      nat.f64(0.0), L.tile_plan(b, 0), self._stream())
         return Y
 
-    def _chebyshev_filter(self, X, m, a, upper):
-        """p_m(L) X, p_m the Chebyshev polynomial of [a, upper] scaled to 1 at 0 (Zhou-Saad)."""
+    def _chebyshev_filter(self, X, m, a, upper, reflect=False):
+        """p_m(L) X, p_m the Chebyshev polynomial of [a, upper] scaled to 1 at 0 (Zhou-Saad).
+        ``reflect``: p_m(upper I - L) X, with alpha A x + beta x = -alpha L x + (alpha upper +
+        beta) x for A = upper I - L."""
         torch = nat.require_cuda()
         L, n, b = self.L, self.n_vertices, X.shape[1]
         plan = L.tile_plan(b, 0)
@@ -254,6 +306,8 @@ class FourierMixIn:
                     gamma = -sigma * sigma_next
                     sigma = sigma_next
                     x_new = x_old            # row-local: x_new may overwrite x_old
+                if reflect:
+                    alpha, beta = -alpha, alpha * upper + beta
                 nat.call("gsp_cheby_step_" + self._sfx, nat.i32(j == 0), nat.i64(0), nat.i64(n),
                          nat.i64(L.nnz), L.indptr, L.indices, L.data, x_cur, x_old, x_new, x_new,
                          nat.i64(n), nat.i64(b), nat.i32(0), zero, zero, nat.f64(alpha),

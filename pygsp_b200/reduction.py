@@ -4,10 +4,11 @@
 of ``pyramid_synthesis`` (:504-514): every step of the Kron pyramid is a Chebyshev filter --
 the analysis filter ``h`` and the order-100 Green kernel ``1 / (eps + x)`` of the
 interpolation -- and runs on the CUDA engine through :class:`pygsp_b200.filters.Filter`.
-What is NOT the filtering path stays host-side set-up, as in the reference: building the
-multiresolution sequence itself (``graph_multiresolution``: eigenvector-based down-sampling,
-Kron reduction, sparsification) and the Schur complement ``K_reg`` of a level
-(:func:`kron_reduction`, a sparse direct solve, computed once per level).
+The multiresolution sequence itself runs on the device too (DESIGN.md section 4.11):
+``graph_multiresolution`` (largest-eigenvector down-sampling by Chebyshev-filtered subspace
+iteration), :func:`kron_reduction` (independent Schur blocks per component of the removed
+vertices, csrc/schur.cu) and :func:`graph_sparsify` (effective resistances from one float64
+factor, seeded Philox sampling).
 
 A graph of the sequence carries ``G.mr = {'idx': kept vertices of the level above,
 'K_reg': ...}`` like the reference's.  Shapes: the reference keeps consistent shapes only for
@@ -19,29 +20,471 @@ reference (NameError at :593) and has no oracle; ``least_squares=True`` raises.
 import numpy as np
 from scipy import sparse
 
+from . import _native as nat
 from . import filters
 from . import utils
 
 logger = utils.build_logger(__name__)
 
 
-def kron_reduction(L, ind):
-    """Kron reduction (Schur complement) of a Laplacian-like sparse matrix onto ``ind``
-    (reduction.py:309-382, matrix branch).  Host-side, once per pyramid level."""
-    from scipy.sparse import linalg
+# Components of the removed vertices with at most SMALL_MAX vertices whose blocks fit in
+# _SMALL_SMEM bytes of shared memory are reduced by the one-CTA kernel (gsp_schur_small_f64);
+# the others by a dense float64 Cholesky (cuSOLVER).  Chosen with tools/multiresolution_probe.py
+# (DESIGN.md section 4.11).
+SMALL_MAX = 64
+_SMALL_SMEM = 96 * 1024
+
+
+def _ctx():
+    torch = nat.require_cuda()
+    return torch, torch.device("cuda:%d" % torch.cuda.current_device())
+
+
+def _device_matrix(L, device):
+    """A host (SciPy / NumPy) or device square matrix as a canonical float64 DeviceCSR without
+    stored zeros: an explicit zero is not an edge (it must not join two components)."""
+    from .graphs.csr import DeviceCSR
+    torch = nat.require_cuda()
+    if isinstance(L, DeviceCSR):
+        M = DeviceCSR(L.indptr, L.indices, L.data.to(torch.float64), L.shape)
+        if bool((M.data == 0).any()):
+            keep = M.data != 0
+            M = _coo_to_csr(M.shape[0], _rows_of(M)[keep], M.indices[keep], M.data[keep])
+        return M
     if hasattr(L, "to_scipy"):
         L = L.to_scipy()
-    L = sparse.csr_matrix(L, dtype=np.float64)
-    n = L.shape[0]
+    host = sparse.csr_matrix(L, dtype=np.float64)
+    if host.shape[0] != host.shape[1]:
+        raise ValueError("The matrix must be square.")
+    host.sum_duplicates()
+    host.eliminate_zeros()
+    host.sort_indices()
+    return DeviceCSR.from_scipy(host, torch.float64, device)
+
+
+def _call(name, *args):
+    nat.call(name, *args, nat.stream_ptr())
+
+
+def _rows_of(M):
+    torch = nat.require_cuda()
+    counts = (M.indptr[1:] - M.indptr[:-1]).long()
+    return torch.repeat_interleave(torch.arange(M.shape[0], device=M.device), counts)
+
+
+def _coo_to_csr(n, rows, cols, vals):
+    """Canonical CSR (duplicates summed in emission order) of float64 COO triplets."""
+    import ctypes
+    from .graphs.csr import DeviceCSR
+    torch = nat.require_cuda()
+    dev = vals.device
+    nnz = int(vals.numel())
+    if nnz >= 2 ** 31:
+        raise ValueError("The result would have {} entries; at most 2^31 - 1 are "
+                         "supported.".format(nnz))
+    indptr = torch.empty(n + 1, dtype=torch.int32, device=dev)
+    indices = torch.empty(nnz, dtype=torch.int32, device=dev)
+    data = torch.empty(nnz, dtype=torch.float64, device=dev)
+    uniq = ctypes.c_int64(0)
+    _call("gsp_coo_to_csr_f64", nat.i64(n), nat.i64(nnz), rows.to(torch.int32).contiguous(),
+          cols.to(torch.int32).contiguous(), vals.contiguous(), indptr, indices, data,
+          ctypes.byref(uniq))
+    m = int(uniq.value)
+    return DeviceCSR(indptr, indices[:m].contiguous(), data[:m].contiguous(), (n, n))
+
+
+def _induced_coo(M, v):
+    """Entries of M[v, :][:, v] as COO (rows, cols, vals) for device int32 ids v."""
+    torch = nat.require_cuda()
+    n, m, dev = M.shape[0], int(v.numel()), M.device
+    mptr = torch.empty(n + 1, dtype=torch.int32, device=dev)
+    mpos = torch.empty(max(m, 1), dtype=torch.int32, device=dev)
+    s_indptr = torch.empty(m + 1, dtype=torch.int32, device=dev)
+    nnz = torch.zeros(1, dtype=torch.int64, device=dev)
+    _call("gsp_vertex_map", nat.i64(n), nat.i64(m), v, mptr, mpos)
+    if m == 0:
+        e = torch.empty(0, dtype=torch.int32, device=dev)
+        return e, e, torch.empty(0, dtype=torch.float64, device=dev), s_indptr.zero_()
+    _call("gsp_subgraph_count", nat.i64(m), M.indptr, M.indices, v, mptr, None, s_indptr, nnz)
+    nnz = int(nnz.item())
+    cols = torch.empty(nnz, dtype=torch.int32, device=dev)
+    vals = torch.empty(nnz, dtype=torch.float64, device=dev)
+    rows = torch.empty(nnz, dtype=torch.int32, device=dev)
+    _call("gsp_subgraph_fill_f64", nat.i64(m), M.indptr, M.indices, M.data, v, mptr, mpos, None,
+          s_indptr, cols, vals, rows)
+    return rows, cols, vals, s_indptr
+
+
+def _schur(M, ind, small_max=None):
+    """Kron reduction of the symmetric float64 DeviceCSR M onto the vertices ``ind`` (host int64
+    array, distinct), as a canonical float64 DeviceCSR in the order of ``ind``.
+
+    M_red - sum_S M_BS M_SS^-1 M_SB over the connected components S of the removed vertices
+    (B: S's kept neighbours): every component is an independent block (csrc/schur.cu).
+    ``small_max`` overrides SMALL_MAX (tests compare the two paths on the same components).
+    """
+    torch = nat.require_cuda()
+    dev, n, m = M.device, M.shape[0], len(ind)
+    small_max = SMALL_MAX if small_max is None else int(small_max)
+    keep = torch.from_numpy(np.ascontiguousarray(ind, dtype=np.int32)).to(dev)
+    slot = torch.zeros(n, dtype=torch.int32, device=dev)
+    slot[keep.long()] = -1 - torch.arange(m, dtype=torch.int32, device=dev)
+    rem = torch.nonzero(slot == 0).flatten().to(torch.int32)
+    r_rows, r_cols, r_vals, _ = _induced_coo(M, keep)
+    nr = int(rem.numel())
+    if nr == 0:
+        return _coo_to_csr(m, r_rows, r_cols, r_vals)
+
+    # components of the removed vertices, listed component by component
+    s_rows, s_cols, s_vals, s_ptr = _induced_coo(M, rem)
+    labels = torch.empty(nr, dtype=torch.int32, device=dev)
+    _call("gsp_cc_labels_f64", nat.i64(nr), s_ptr, s_cols, s_vals, nat.i32(0), labels, None)
+    perm = torch.empty(nr, dtype=torch.int32, device=dev)
+    cptr = torch.empty(nr + 1, dtype=torch.int32, device=dev)
+    ncomp = torch.empty(1, dtype=torch.int64, device=dev)
+    _call("gsp_component_order", nat.i64(nr), labels, perm, cptr, ncomp)
+    nc = int(ncomp.item())
+    cptr = cptr[:nc + 1].contiguous()
+    cvert = rem[perm.long()].contiguous()
+    sizes = (cptr[1:] - cptr[:-1]).long()
+    comp_of_pos = torch.repeat_interleave(torch.arange(nc, device=dev), sizes)
+    slot[cvert.long()] = (torch.arange(nr, device=dev) - cptr[comp_of_pos].long()).to(torch.int32)
+    comp_of = torch.full((n,), -1, dtype=torch.int64, device=dev)
+    comp_of[cvert.long()] = comp_of_pos
+
+    # kept neighbours of every component, in increasing kept index
+    rows, cols = _rows_of(M), M.indices.long()
+    edge = (comp_of[rows] >= 0) & (slot[cols] < 0)
+    keys = torch.unique(comp_of[rows[edge]] * m + (-1 - slot[cols[edge]].long()))
+    bcomp, bidx = keys // m, (keys % m).to(torch.int32).contiguous()
+    nbs = torch.bincount(bcomp, minlength=nc)
+    bptr = torch.zeros(nc + 1, dtype=torch.int64, device=dev)
+    bptr[1:] = torch.cumsum(nbs, 0)
+    out_len = nbs * nbs
+    out_off = torch.zeros(nc + 1, dtype=torch.int64, device=dev)
+    out_off[1:] = torch.cumsum(out_len, 0)
+    total = int(out_off[-1].item())
+    nnz_red = int(r_vals.numel())
+    if total + nnz_red >= 2 ** 31:
+        raise ValueError("The Kron reduction would have {} entries before summation; at most "
+                         "2^31 - 1 are supported.".format(total + nnz_red))
+
+    # small components: one CTA each; the others: dense Cholesky.  A component without kept
+    # neighbours contributes nothing (its M_SS may be singular) and is skipped.
+    smem = 8 * (sizes * sizes + sizes + sizes * nbs) + 4 * nbs
+    small = (sizes <= small_max) & (smem <= _SMALL_SMEM) & (nbs > 0)
+    dense = (~small) & (nbs > 0)
+    rows_out = torch.empty(total + nnz_red, dtype=torch.int32, device=dev)
+    cols_out = torch.empty(total + nnz_red, dtype=torch.int32, device=dev)
+    vals_out = torch.empty(total + nnz_red, dtype=torch.float64, device=dev)
+    rows_out[total:], cols_out[total:], vals_out[total:] = r_rows, r_cols, r_vals
+    status = torch.zeros(1, dtype=torch.int32, device=dev)
+    bptr32 = bptr.to(torch.int32).contiguous()
+    comps = torch.nonzero(small).flatten().to(torch.int32).contiguous()
+    if comps.numel():
+        _call("gsp_schur_small_f64", M.indptr, M.indices, M.data, slot, cvert, cptr, bptr32, bidx,
+              nat.i64(comps.numel()), comps, nat.i32(int(smem[small].max().item())),
+              out_off, rows_out, cols_out, vals_out, status)
+    dense_ids = torch.nonzero(dense).flatten().cpu().numpy()
+    if dense_ids.size:
+        host_c, host_b, host_o = (cptr.cpu().numpy(), bptr.cpu().numpy(),
+                                  out_off.cpu().numpy())
+        for c in dense_ids:
+            c0, s = int(host_c[c]), int(host_c[c + 1] - host_c[c])
+            b0, b = int(host_b[c]), int(host_b[c + 1] - host_b[c])
+            A = torch.empty((s, s), dtype=torch.float64, device=dev)
+            B = torch.empty((s, b), dtype=torch.float64, device=dev)
+            bc = bidx[b0:b0 + b]
+            _call("gsp_schur_gather_f64", M.indptr, M.indices, M.data, slot, cvert[c0:c0 + s],
+                  nat.i64(s), bc, nat.i64(b), A, B)
+            C, info = torch.linalg.cholesky_ex(A)
+            if int(info.item()) != 0:
+                status.fill_(1)
+                continue
+            Y = torch.linalg.solve_triangular(C, B, upper=False)
+            del A, B, C
+            K = Y.T @ Y
+            o = int(host_o[c])
+            vals_out[o:o + b * b] = (-0.5 * (K + K.T)).flatten()
+            rows_out[o:o + b * b] = bc.repeat_interleave(b)
+            cols_out[o:o + b * b] = bc.repeat(b)
+    if int(status.item()):
+        raise ValueError("Kron reduction: a block of the removed vertices is not positive "
+                         "definite (the matrix is not a connected Laplacian-like matrix).")
+    # components without kept neighbours emitted nothing: their slots are empty (b = 0)
+    out = _coo_to_csr(m, rows_out, cols_out, vals_out)
+    # Every block is symmetric and M_red is, but the summation of duplicates need not associate
+    # (i, j) and (j, i) alike; average with the transpose if any entry differs (the reference
+    # symmetrises an almost symmetric result too, reduction.py:361-362).
+    if _asymmetry(out):
+        from .graphs.graph import symmetrize_average_device
+        out = symmetrize_average_device(out)
+    return out
+
+
+def _asymmetry(M):
+    """Number of stored entries of the float64 DeviceCSR M that differ from their transpose."""
+    torch = nat.require_cuda()
+    count = torch.zeros(1, dtype=torch.int64, device=M.device)
+    _call("gsp_csr_asymmetry_f64", nat.i64(M.shape[0]), M.indptr, M.indices, M.data, count)
+    return int(count.item())
+
+
+def _check_symmetric(M):
+    if _asymmetry(M):
+        raise ValueError("Kron reduction on the device needs a symmetric matrix.")
+
+
+def _kept_ids(ind, n):
     ind = np.asarray(ind)
-    rest = np.setdiff1d(np.arange(n, dtype=int), ind)
-    inner = L[rest][:, rest].tocsc()
-    coupling = L[rest][:, ind].tocsc()
-    schur = L[ind][:, ind] - L[ind][:, rest].dot(linalg.spsolve(inner, coupling))
-    schur = sparse.csr_matrix(schur)
-    if np.abs(schur - schur.T).sum() < np.spacing(1) * np.abs(schur).sum():
-        schur = (schur + schur.T) / 2.0
-    return sparse.csr_matrix(schur)
+    if ind.dtype == bool:
+        ind = np.flatnonzero(ind)
+    ind = ind.astype(np.int64).reshape(-1)
+    if ind.size and (ind.min() < 0 or ind.max() >= n or np.unique(ind).size != ind.size):
+        raise ValueError("ind must list distinct vertices in [0, {}).".format(n))
+    return ind
+
+
+def kron_reduction(G, ind):
+    r"""Compute the Kron reduction (reduction.py:309-382).
+
+    ``G``: a :class:`Graph` with a combinatorial Laplacian, or a symmetric sparse matrix
+    (Laplacian-like, such as ``L + eps I``; SciPy, NumPy or a ``DeviceCSR``).  Unlike the
+    reference, a non-symmetric matrix raises ``ValueError`` (each block is factored by Cholesky),
+    and so does a matrix whose removed blocks are not positive definite.  ``ind``: the
+    vertices to keep, in the order of the result.  The Schur complement
+    ``L[ind, ind] - L[ind, comp] L[comp, comp]^-1 L[comp, ind]`` is computed on the device in
+    float64, one independent block per connected component of the removed vertices
+    (csrc/schur.cu).  A matrix in gives a SciPy CSR float64 matrix out; a graph in gives a graph
+    on ``W = -offdiag(L_new)`` with the sliced coordinates, in the graph's dtype (weights that
+    underflow in float32 are dropped).  The diagonal of ``L_new`` is dropped, as the reference's
+    comment intends; its ``Snew`` correction (reduction.py:366-372) is not reproduced (DESIGN.md
+    section 2).
+    """
+    from .graphs import Graph
+    torch = nat.require_cuda()
+    if isinstance(G, Graph):
+        if G.lap_type != "combinatorial":
+            raise NotImplementedError("Unknown reduction for {} Laplacian.".format(G.lap_type))
+        if G.is_directed():
+            raise NotImplementedError("This method only work for undirected graphs.")
+        ind = _kept_ids(ind, G.N)
+        with torch.cuda.device(G.device):
+            L = _schur(_device_matrix(G.L, G.device), ind)
+            rows = _rows_of(L)
+            off = rows != L.indices.long()
+            Gnew = Graph.from_coo(rows[off], L.indices[off], -L.data[off], len(ind),
+                                  lap_type=G.lap_type, dtype=G.dtype, device=G.device,
+                                  coords=G.coords[ind] if hasattr(G, "coords") else None,
+                                  plotting=G.plotting)
+        return Gnew
+    _, dev = _ctx()
+    M = _device_matrix(G, dev)
+    _check_symmetric(M)
+    ind = _kept_ids(ind, M.shape[0])
+    return _schur(M, ind).to_scipy().astype(np.float64)
+
+
+def _laplacian_inverse(L):
+    """(Ainv, labels, sizes) for a float64 Laplacian DeviceCSR: Ainv = (L + sum_c 1_c 1_c^T / |c|)^-1
+    = L^+ + sum_c 1_c 1_c^T / |c| (dense, float64, on the device), by one Cholesky factor.
+    labels: component of every vertex (smallest vertex id), sizes[v] = |component of v|."""
+    torch = nat.require_cuda()
+    n, dev = L.shape[0], L.device
+    labels = torch.empty(n, dtype=torch.int32, device=dev)
+    _call("gsp_cc_labels_f64", nat.i64(n), L.indptr, L.indices, L.data, nat.i32(0), labels, None)
+    lab = labels.long()
+    sizes = torch.bincount(lab, minlength=n)[lab].double()
+    free, _ = torch.cuda.mem_get_info(dev)
+    if 3 * n * n * 8 > free:
+        raise ValueError("The dense factor of this {0} x {0} Laplacian needs about {1:.1f} GB of "
+                         "device memory ({2:.1f} GB free).".format(n, 3 * n * n * 8 / 2 ** 30,
+                                                                  free / 2 ** 30))
+    A = torch.zeros((n, n), dtype=torch.float64, device=dev)
+    A[_rows_of(L), L.indices.long()] = L.data
+    step = max(1, (1 << 26) // max(n, 1))
+    for r0 in range(0, n, step):
+        r1 = min(n, r0 + step)
+        A[r0:r1] += (lab[r0:r1, None] == lab[None, :]) / sizes[r0:r1, None]
+    C, info = torch.linalg.cholesky_ex(A)
+    del A
+    if int(info.item()) != 0:
+        raise ValueError("The matrix is not a combinatorial Laplacian (its Cholesky factor "
+                         "does not exist).")
+    return torch.cholesky_inverse(C), lab, sizes
+
+
+def resistance_distance(M):
+    r"""Resistance distances of a graph (utils.py:140-181), a dense (N, N) float64 ndarray.
+
+    ``M``: a :class:`Graph` with a combinatorial Laplacian, or a Laplacian as a sparse matrix.
+    ``R_uv = L+_uu + L+_vv - 2 L+_uv`` with the pseudo-inverse ``L+`` from one float64 Cholesky
+    factor of ``L + sum_c 1_c 1_c^T / |c|`` (one rank-one term per connected component), on the
+    device.  The reference inverts the singular L with SuperLU and falls back to ``pinv`` only
+    when SuperLU reports the singularity; this is exact.  Vertices of different components get
+    ``L+_uu + L+_vv``, as with ``pinv``.
+    """
+    from .graphs import Graph
+    torch, dev = _ctx()
+    if isinstance(M, Graph):
+        if M.lap_type != "combinatorial":
+            raise ValueError("Need a combinatorial Laplacian.")
+        dev, L = M.device, M.L
+    else:
+        L = M
+    with torch.cuda.device(dev):
+        Ainv, lab, sizes = _laplacian_inverse(_device_matrix(L, dev))
+        n = Ainv.shape[0]
+        step = max(1, (1 << 26) // max(n, 1))
+        for r0 in range(0, n, step):
+            r1 = min(n, r0 + step)
+            Ainv[r0:r1] -= (lab[r0:r1, None] == lab[None, :]) / sizes[r0:r1, None]
+        d = torch.diagonal(Ainv).clone()
+        R = d[:, None] + d[None, :] - Ainv - Ainv.T
+        return R.cpu().numpy()
+
+
+def _sampling_seed(seed, i):
+    return (int(0 if seed is None else seed) * 0x9E3779B97F4A7C15 + i) & 0xFFFFFFFFFFFFFFFF
+
+
+def graph_sparsify(M, epsilon, maxiter=10, seed=None):
+    r"""Sparsify a graph with Spielman-Srivastava (reduction.py:34-147).
+
+    ``M``: a :class:`Graph` (combinatorial Laplacian, else ``NotImplementedError``) or a
+    Laplacian as a sparse matrix; ``epsilon`` in ``[1/sqrt(N), 1)`` (else ``ValueError``).
+    ``q = round(9 C^2 N log N / epsilon^2)`` edges are drawn with probability ``P_e`` proportional
+    to ``w_e R_e`` (``R_e`` the edge's effective resistance, from one float64 Cholesky factor on
+    the device), and an edge drawn ``k`` times gets the weight ``k w_e / (q P_e)``.  If the result
+    is disconnected, epsilon is lowered and the sampling repeated, at most ``maxiter`` times.
+
+    Differences from the reference (DESIGN.md section 2): the draws come from counter-based
+    Philox streams of ``seed`` (``None`` means 0), so the same seed gives the same bits but not
+    SciPy's draws; ``P_e`` is ``w_e R_e`` rounded to 32 bits relative to its largest value (the
+    distribution actually sampled); per-edge counts stand for the removed ``stats.itemfreq``; the
+    graph keeps its coordinates; a matrix in gives the Laplacian ``D' - W'`` as a SciPy CSR matrix
+    out (the reference returns ``-W'`` as a ``lil_matrix``).
+    """
+    from .graphs import Graph
+    torch, dev = _ctx()
+    is_graph = isinstance(M, Graph)
+    if is_graph:
+        if not M.lap_type == "combinatorial":
+            raise NotImplementedError
+        dev, L, N = M.device, M.L, M.N
+    else:
+        L, N = M, np.shape(M)[0]
+    if not 1.0 / np.sqrt(N) <= epsilon < 1:
+        raise ValueError("GRAPH_SPARSIFY: Epsilon out of required range")
+
+    with torch.cuda.device(dev):
+        Ld = _device_matrix(L, dev)
+        rows, cols = _rows_of(Ld), Ld.indices.long()
+        w = -Ld.data
+        # edges: the lower triangle of W with w >= 1e-10 (reduction.py:89-97)
+        edge = (rows > cols) & (w >= 1e-10)
+        start, end, weights = rows[edge], cols[edge], w[edge].contiguous()
+        ne = int(weights.numel())
+        Ainv, _, _ = _laplacian_inverse(Ld)
+        R = torch.empty(ne, dtype=torch.float64, device=dev)
+        e32 = [x.to(torch.int32).contiguous() for x in (start, end)]
+        _call("gsp_edge_resistance_f64", nat.i64(ne), e32[0], e32[1], Ainv, nat.i64(N), R)
+        del Ainv
+        x = weights * torch.clamp(R, min=0)
+        xmax = float(x.max().item()) if ne else 0.0
+        if not xmax > 0:
+            raise ValueError("GRAPH_SPARSIFY: the graph has no edge with a positive weight")
+        k = torch.round(x / xmax * 2.0 ** 32).to(torch.int64).contiguous()
+        total = int(k.sum().item())
+        Pe = k.double() / total
+        counts = torch.empty(ne, dtype=torch.int64, device=dev)
+        for i in range(maxiter):
+            C0 = 1 / 30.0
+            C = 4 * C0
+            q = int(round(N * np.log(N) * 9 * C ** 2 / (epsilon ** 2)))
+            _call("gsp_sparsify_sample", nat.i64(ne), k, nat.i64(q), nat.u64(_sampling_seed(seed, i)),
+                  counts)
+            hit = counts > 0
+            new_w = counts[hit].double() * weights[hit] / (q * Pe[hit])
+            r, c = start[hit], end[hit]
+            sparser = Graph.from_coo(torch.cat([r, c]), torch.cat([c, r]), torch.cat([new_w, new_w]),
+                                     N, dtype=torch.float64, device=dev)
+            if sparser.is_connected():
+                break
+            elif i == maxiter - 1:
+                logger.warning("Despite attempts to reduce epsilon, sparsified graph is "
+                               "disconnected")
+            else:
+                epsilon -= (epsilon - 1 / np.sqrt(N)) / 2.0
+        if is_graph:
+            W = sparser.W
+            return Graph(W, lap_type=M.lap_type, coords=getattr(M, "coords", None),
+                         plotting=M.plotting, dtype=M.dtype, device=dev)
+        sparser.compute_laplacian("combinatorial")
+        return sparser.L.to_scipy().astype(np.float64)
+
+
+def graph_multiresolution(G, levels, sparsify=True, sparsify_eps=None,
+                          downsampling_method="largest_eigenvector", reduction_method="kron",
+                          compute_full_eigen=False, reg_eps=0.005, *, seed=0):
+    r"""Compute a pyramid of graphs by Kron reduction (reduction.py:196-306).
+
+    Per level: the eigenvector ``V`` of the largest eigenvalue of L (``G._largest_eigenvector``,
+    on the device), ``V *= sign(V[0])``, keep ``ind = V >= 0``, Kron-reduce onto ``ind``
+    (:func:`kron_reduction`), then, with ``sparsify``, :func:`graph_sparsify` with epsilon
+    ``min(max(sparsify_eps, 2 / sqrt(N)), 1)``; then ``estimate_lmax()`` (or the full Fourier
+    basis with ``compute_full_eigen``).  ``Gs[i + 1].mr = {'idx', 'orig_idx', 'level'}`` and, on
+    the level above, ``mr['K_reg']`` (Kron reduction of ``L + reg_eps I``, a SciPy CSR matrix) and
+    ``mr['green_kernel']``, as in the reference.  ``seed`` seeds the eigenvector solver and the
+    sparsification of every level.
+    """
+    if sparsify_eps is None:
+        sparsify_eps = min(10.0 / np.sqrt(G.N), 0.3)
+    if compute_full_eigen:
+        G.compute_fourier_basis()
+    else:
+        G.estimate_lmax()
+    Gs = [G]
+    Gs[0].mr = {"idx": np.arange(G.N), "orig_idx": np.arange(G.N)}
+    for i in range(levels):
+        if downsampling_method == "largest_eigenvector":
+            V = Gs[i]._largest_eigenvector(seed=seed)
+            V *= np.sign(V[0])
+            ind = np.nonzero(V >= 0)[0]
+        else:
+            raise NotImplementedError("Unknown graph downsampling method.")
+        if reduction_method == "kron":
+            Gs.append(kron_reduction(Gs[i], ind))
+        else:
+            raise NotImplementedError("Unknown graph reduction method.")
+        if sparsify and Gs[i + 1].N > 2:
+            Gs[i + 1] = graph_sparsify(Gs[i + 1], min(max(sparsify_eps, 2.0 / np.sqrt(Gs[i + 1].N)),
+                                                      1.0), seed=_sampling_seed(seed, 1000 + i))
+        if compute_full_eigen:
+            Gs[i + 1].compute_fourier_basis()
+        else:
+            Gs[i + 1].estimate_lmax()
+        Gs[i + 1].mr = {"idx": ind, "orig_idx": Gs[i].mr["orig_idx"][ind], "level": i}
+        Gs[i].mr["K_reg"] = _kron_regularized(Gs[i], ind, reg_eps)
+        Gs[i].mr["_kreg_key"] = (reg_eps, ind.tobytes())
+        Gs[i].mr["green_kernel"] = filters.Filter(Gs[i], lambda x: 1.0 / (reg_eps + x))
+        Gs[i].mr["_green_eps"] = reg_eps
+    return Gs
+
+
+def _kron_regularized(G, ind, reg_eps):
+    """Kron reduction of L + reg_eps I onto ind (reduction.py:302-303), L + reg_eps I assembled
+    on the device."""
+    torch = nat.require_cuda()
+    with torch.cuda.device(G.device):
+        L = _device_matrix(G.L, G.device)
+        n = G.N
+        diag = torch.arange(n, dtype=torch.int32, device=G.device)
+        M = _coo_to_csr(n, torch.cat([_rows_of(L).to(torch.int32), diag]),
+                        torch.cat([L.indices, diag]),
+                        torch.cat([L.data, torch.full((n,), float(reg_eps), dtype=torch.float64,
+                                                      device=G.device)]))
+        return _schur(M, ind).to_scipy().astype(np.float64)
 
 
 def _as_columns(s):

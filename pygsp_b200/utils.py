@@ -38,6 +38,17 @@ def compute_log_scales(lmin, lmax, Nscales, t1=1, t2=2):
     return np.exp(np.linspace(np.log(t2 / lmin), np.log(t1 / lmax), Nscales))
 
 
+def resistance_distance(G):
+    r"""Resistance distances of a graph (pygsp/utils.py:140-181): a dense (N, N) float64 ndarray.
+
+    ``G``: a :class:`pygsp_b200.graphs.Graph` with a combinatorial Laplacian (else
+    ``ValueError``) or a Laplacian as a sparse matrix.  Computed on the device from one float64
+    Cholesky factor (:func:`pygsp_b200.reduction.resistance_distance`).
+    """
+    from .reduction import resistance_distance as _device_resistance_distance
+    return _device_resistance_distance(G)
+
+
 def symmetrize(W, method="average"):
     """Host-side symmetrisation used by the graph generators (pygsp/utils.py:184-277).
 
