@@ -214,6 +214,37 @@ int gsp_lanczos_f64(int64_t n, int64_t nnz, const int32_t* indptr, const int32_t
 GSPB200_DECLARE_CG_API(f32, float)
 GSPB200_DECLARE_CG_API(f64, double)
 
+/* gsp_fb_simplex_*: accelerated forward-backward (FISTA) for
+ *   min_X tau tr(X^T L X) + ||M (X - Y)||^2  s.t. every row of X on the probability simplex,
+ *   Y the one-hot (n, nclass) matrix of the labels -- pyunlocbox's forward_backward + solve on the
+ *   problem of pygsp/learning.py:42-180 (classification_tikhonov_simplex), started from X = Y.
+ *   label (n, int32): class of a labelled vertex, -1 where M is False; 1 <= nclass <= 256.
+ *   step: the gradient step (the reference's 0.5 / (1 + tau lmax)).  Runs iterations
+ *   [it0, it1) (it0 == 0 writes X = Y and resets the state); an iteration is the SpMM L X_k
+ *   (gsp_cheby_step_*, tiled where plan_host applies) and one row pass that forms the
+ *   extrapolated point, its gradient (L y by linearity: no second SpMM), projects every row onto
+ *   the simplex (Michelot, sort-free) and adds up the objective of X_k in a fixed order.  X2 and
+ *   LX2 each hold two (n, nclass) row-major blocks; iterate k is X2 block k % 2.
+ *   Stop tests of pyunlocbox.solvers.solve, on iterate k >= 1 with objective f_k:
+ *   tol_host = {atol, dtol, rtol, xtol} (host doubles, NaN = off), maxit < 0 = off;
+ *   f_k < atol | |f_k - f_{k-1}| < dtol | |f_k - f_{k-1}| / |f_k| < rtol (f_{k-1} when f_k = 0,
+ *   ratio 0 when both are) | ||X_k - X_{k-1}|| / sqrt(n nclass) < xtol | k >= maxit; the last
+ *   one that holds names the stop.  Once one holds, later row passes do nothing, so the state
+ *   stays at the stopping iterate however far past it the caller enqueued.  scal_dev holds
+ *   GSPB200_FB_HISTORY + cap doubles (it1 <= cap): [1] the stop criterion (0 = running,
+ *   1 atol, 2 dtol, 3 rtol, 4 xtol, 5 maxit), [2] the stop iteration, and from
+ *   GSPB200_FB_HISTORY on the objective f_k of every iterate, which the host reads. */
+#define GSPB200_FB_HISTORY 3080
+#define GSPB200_DECLARE_FB_API(SUF, T)                                                           \
+  int gsp_fb_simplex_##SUF(int64_t n, int64_t nnz, const int32_t* indptr, const int32_t* indices, \
+                           const T* data, const int32_t* label, int64_t nclass, double tau,       \
+                           double step, const double* tol_host, int maxit, T* X2, T* LX2,         \
+                           int it0, int it1, int cap, double* scal_dev,                           \
+                           const gsp_tile_plan* plan_host, void* stream);
+
+GSPB200_DECLARE_FB_API(f32, float)
+GSPB200_DECLARE_FB_API(f64, double)
+
 /* --------------------------------------------------------- spectral basis ---
  * Tall-skinny block kernels of the graph Fourier basis (pygsp_b200/graphs/fourier.py): gft /
  * igft and the partial eigensolver that stands for scipy's eigsh (Chebyshev-filtered subspace

@@ -6,6 +6,10 @@ time in a Python loop, every product a SciPy SpMV (learning.py:326-337); for ``t
 solves the harmonic extension ``L_uu x_u = -L_ul y_l`` with a sparse direct solver (:350-365).
 Here both are ONE block conjugate-gradient run on the device (``gsp_cg_*``, csrc/cg.cu): all
 columns advance together, the product with L is the SpMM step kernel of the filter path.
+
+``classification_tikhonov_simplex`` (learning.py:42-180) hands its problem to pyunlocbox's
+accelerated forward-backward solver; here that solver runs on the device (``gsp_fb_simplex_*``,
+csrc/simplex.cu) with its stopping rules, and pyunlocbox is not needed.
 """
 import numpy as np
 
@@ -13,6 +17,17 @@ from . import _native as nat
 from . import utils
 
 logger = utils.build_logger(__name__)
+
+# iterations enqueued between two reads of the simplex solver's stop record
+SIMPLEX_BATCH = 16
+MAX_CLASSES = 256
+_FB_HISTORY = 3080                      # GSPB200_FB_HISTORY (include/gspb200.h)
+_CRITS = {1: "ATOL", 2: "DTOL", 3: "RTOL", 4: "XTOL", 5: "MAXIT"}
+_SOLVE_DEFAULTS = {"atol": None, "dtol": None, "rtol": 1e-3, "xtol": None, "maxit": 200,
+                   "verbosity": "LOW"}
+
+# the last classification_tikhonov_simplex run: {'niter', 'crit', 'objective', 'batches'}
+last_solve = None
 
 
 def _to_logits(x):
@@ -27,6 +42,100 @@ def classification_tikhonov(G, y, M, tau=0):
     y[np.asarray(M) == False] = 0  # noqa: E712
     Y = _to_logits(y.astype(int))
     return regression_tikhonov(G, Y, M, tau)
+
+
+def classification_tikhonov_simplex(G, y, M, tau=0.1, **kwargs):
+    r"""Classification with class probabilities by Tikhonov minimisation (learning.py:42-180).
+
+    ``argmin_X ||M X - Y||^2 + tau tr(X'LX)`` with every row of X on the probability simplex
+    (``X >= 0``, rows summing to 1), Y the one-hot logits of the labels ``y`` (C = max label + 1
+    classes, at most 256).  Solved by accelerated forward-backward (FISTA) from ``X = Y`` with
+    step ``0.5 / (1 + tau G.lmax)``, as the reference does with pyunlocbox.  ``y``: (N,)
+    measurements (entries where ``M`` is False are ignored and may be NaN), ``M``: boolean mask
+    of length N; the inputs are not modified.  Keywords are pyunlocbox's ``solve`` stopping
+    parameters: ``atol``, ``dtol``, ``rtol`` (default 1e-3), ``xtol``, ``maxit`` (default 200)
+    and ``verbosity`` ('NONE', 'LOW', 'HIGH', 'ALL': what is logged).  Returns the (N, C) X;
+    NumPy in -> NumPy out (float64 for a float64 graph, else float32), CUDA tensor in -> CUDA
+    tensor out.  ``learning.last_solve`` then holds the iteration count, the stopping criterion
+    and the objective at every iterate.
+    """
+    global last_solve
+    unknown = sorted(set(kwargs) - set(_SOLVE_DEFAULTS))
+    if unknown:
+        raise TypeError("classification_tikhonov_simplex() got an unexpected keyword argument "
+                        "'%s'" % unknown[0])
+    if tau <= 0:
+        raise ValueError("Tau should be greater than 0.")
+    opts = dict(_SOLVE_DEFAULTS, **kwargs)
+    if opts["verbosity"] not in ("NONE", "LOW", "HIGH", "ALL"):
+        raise ValueError("Verbosity should be either NONE, LOW, HIGH or ALL.")
+    if all(opts[k] is None for k in ("atol", "dtol", "rtol", "xtol", "maxit")):
+        raise ValueError("at least one stopping criterion (atol, dtol, rtol, xtol, maxit) is needed")
+    torch = nat.require_cuda()
+    is_tensor = torch.is_tensor(y)
+    M_host = np.asarray(M.cpu() if torch.is_tensor(M) else M)
+    if M_host.size != G.n_vertices:
+        raise ValueError("M should be of size [G.n_vertices,]")
+    mask = torch.as_tensor(M_host.astype(bool).ravel(), device=G.device)
+    yt = (y if is_tensor else torch.as_tensor(np.asarray(y, dtype=np.float64))).to(
+        device=G.device, dtype=torch.float64).reshape(-1)
+    if yt.numel() != G.n_vertices:
+        raise ValueError("y should be of size [G.n_vertices,]")
+    yt = torch.where(mask, yt, torch.zeros_like(yt))         # learning.py:117 (NaNs dropped)
+    if bool(torch.isnan(yt).any()):
+        raise ValueError("labelled vertices must have a label (got NaN)")
+    lab = yt.to(torch.int64)                                 # y.astype(int): toward zero
+    if bool((lab < 0).any()):
+        raise ValueError("labels must be non-negative integers")
+    C = int(lab.max()) + 1
+    if C > MAX_CLASSES:
+        raise ValueError("at most %d classes are supported, got %d" % (MAX_CLASSES, C))
+    label = torch.where(mask, lab, torch.full_like(lab, -1)).to(torch.int32).contiguous()
+
+    step = 0.5 / (1 + tau * G.lmax)
+    n, L = G.n_vertices, G.L
+    maxit = opts["maxit"]
+    # iteration k's objective is formed by the k-th row pass: maxit stops by pass max(maxit, 1)
+    last_pass = None if maxit is None else max(int(maxit), 1)
+    cap = last_pass + 1 if last_pass is not None else 1024
+    tol = np.array([np.nan if opts[k] is None else float(opts[k])
+                    for k in ("atol", "dtol", "rtol", "xtol")], dtype=np.float64)
+    X2 = torch.empty(2 * n * C, dtype=G.dtype, device=G.device)
+    LX2 = torch.empty_like(X2)
+    plan = L.tile_plan(C, 0)
+    with torch.cuda.device(G.device):
+        scal = torch.zeros(_FB_HISTORY + cap, dtype=torch.float64, device=G.device)
+        done, batches = 0, 0
+        while True:
+            nxt = done + SIMPLEX_BATCH
+            if last_pass is not None:
+                nxt = min(nxt, last_pass + 1)
+            elif nxt > cap:                                  # maxit=None: grow the history
+                cap = max(2 * cap, nxt)
+                scal = torch.cat([scal, scal.new_zeros(_FB_HISTORY + cap - scal.numel())])
+            nat.call("gsp_fb_simplex_" + nat.suffix(G.dtype), nat.i64(n), nat.i64(L.nnz),
+                     L.indptr, L.indices, L.data, label, nat.i64(C), nat.f64(tau), nat.f64(step),
+                     tol, nat.i32(-1 if maxit is None else maxit), X2, LX2, nat.i32(done),
+                     nat.i32(nxt), nat.i32(cap), scal, plan, nat.stream_ptr(G.device))
+            done, batches = nxt, batches + 1
+            rec = scal[:3].cpu().numpy()
+            if rec[1] != 0:
+                break
+            if last_pass is not None and done > last_pass:
+                raise nat.NativeError("the simplex solver did not stop at maxit")
+    niter, crit = int(rec[2]), _CRITS[int(rec[1])]
+    obj = scal[_FB_HISTORY:_FB_HISTORY + niter + 1].cpu().numpy()
+    last_solve = {"niter": niter, "crit": crit, "objective": obj, "batches": batches}
+    if opts["verbosity"] in ("HIGH", "ALL"):
+        for k in range(1, niter + 1):
+            logger.info("iteration %d: objective = %.2e", k, obj[k])
+    if opts["verbosity"] != "NONE":
+        logger.info("Solution found after %d iterations: objective f(sol) = %e, stopping "
+                    "criterion: %s", niter, obj[-1], crit)
+    X = X2[(niter % 2) * n * C:(niter % 2 + 1) * n * C].reshape(n, C).clone()
+    if is_tensor:
+        return X
+    return X.cpu().numpy().astype(np.float64 if G.dtype == torch.float64 else np.float32)
 
 
 def _block_cg(G, tau, row_scale, diag, B, tol, maxiter):
