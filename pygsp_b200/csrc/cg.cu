@@ -12,8 +12,7 @@
 //   apply     Q = a.Q + d.P ; partial sums of P.Q per column
 //   update    alpha = rr/pq ; X += alpha P ; R -= alpha Q ; partial sums of R.R
 //   direction beta = rr'/rr ; P = R + beta P ; rr history[it+1] = rr'
-#include "common.cuh"
-#include "gspb200.h"
+#include "step.cuh"
 
 namespace gsp {
 
@@ -164,10 +163,15 @@ int cg_run(int64_t n, int64_t nnz, const int32_t* indptr, const int32_t* indices
     note_launch(1);
     GSP_LAUNCH_CHECK("cg_init");
   }
-  double zero = 0;
+  Step<T> spmm{nnz, indptr, indices, data};       // Q = tau L P: the first form, no r_i
+  spmm.x_cur = P;
+  spmm.x_new = spmm.r = Q;
+  spmm.r_rows = n;
+  spmm.nsig = nsig;
+  spmm.first = true;
+  spmm.alpha = tau;
   for (int it = it0; it < it1; ++it) {
-    int rc = cheby_step<T>(true, 0, n, indptr, indices, data, P, nullptr, Q, Q, n, nsig, 0, &zero,
-                           &zero, tau, 0.0, 0.0, st);
+    int rc = run_step<T>(spmm, 0, n, nullptr, nullptr, st);
     if (rc != GSP_OK) return rc;
     cg_apply_kernel<T><<<s.blocks, kCgThreads, 0, st>>>(n, nsig, s.cw, a_row, d_row, P, Q, part_pq);
     cg_update_kernel<T><<<s.blocks, kCgThreads, 0, st>>>(n, nsig, s.cw, X, R, P, Q,

@@ -21,29 +21,10 @@
 // gathers its packet of x_cur[col] -- a 16*G-byte contiguous, fully coalesced
 // request per neighbour -- and accumulates in registers.  The accumulation
 // order is the stored CSR order, i.e. the order scipy uses.
-#include "common.cuh"
-#include "gspb200.h"
+#include "step.cuh"
 
 namespace gsp {
 
-int cheby_step_tiled_f32(bool first, int64_t rb, int64_t re, int64_t nnz, const int32_t* indptr,
-                         const int32_t* indices, const float* vals, const float* x_cur,
-                         const float* x_old, float* x_new, float* r, int64_t r_rows, int nsig,
-                         int nscales, const double* ck, const double* c0, double alpha, double beta,
-                         double gamma, const gsp_tile_plan& plan, const gsp_halo_fusion* halo,
-                         int64_t* rows_done, cudaStream_t st, bool add_source = false,
-                         bool reverse = false, const int64_t* out_perm = nullptr);
-int cheby_step_tiled_halo_f32(bool first, int64_t n, int64_t nnz, const int32_t* indptr,
-                              const int32_t* indices, const float* vals, const float* x_cur,
-                              const float* x_old, float* x_new, float* r, int64_t r_rows, int nsig,
-                              int nscales, const double* ck, const double* c0, double alpha,
-                              double beta, double gamma, const gsp_tile_plan& plan,
-                              const gsp_halo_fusion& halo, int64_t* rows_done, cudaStream_t st,
-                              bool add_source, bool reverse, const int64_t* out_perm);
-
-static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
-
-constexpr int kMaxScales = 16;   // coefficients per launch passed by value
 constexpr int kStepThreads = 256;
 
 template <typename T>
@@ -223,36 +204,33 @@ template <> struct MaxVec<float> { static constexpr int value = 4; };
 template <> struct MaxVec<double> { static constexpr int value = 2; };
 
 
-// One recurrence step over rows [rb, re).  Handles any nsig / nscales.
 template <typename T>
-int cheby_step(bool first, int64_t rb, int64_t re, const int32_t* indptr,
-               const int32_t* indices, const T* vals, const T* x_cur, const T* x_old,
-               T* x_new, T* r, int64_t r_rows, int nsig, int nscales, const double* ck,
-               const double* c0, double alpha, double beta, double gamma, cudaStream_t st,
-               bool add_source, const int64_t* out_perm) {
+int cheby_step(const Step<T>& s, int64_t rb, int64_t re, cudaStream_t st) {
   constexpr int MV = MaxVec<T>::value;
-  const bool vec_ok = (nsig % MV == 0) && aligned16(x_cur) && aligned16(x_new) &&
-                      aligned16(r) && (first || aligned16(x_old));
-  for (int s0 = 0; s0 < nscales || s0 == 0; s0 += kMaxScales) {
-    const int ns = min(kMaxScales, nscales - s0);
+  const int nsig = s.nsig;
+  const bool vec_ok = (nsig % MV == 0) && aligned16(s.x_cur) && aligned16(s.x_new) &&
+                      aligned16(s.r) && (s.first || aligned16(s.x_old));
+  for (int s0 = 0; s0 < s.nscales || s0 == 0; s0 += kMaxScales) {
+    const int ns = min(kMaxScales, s.nscales - s0);
     StepCoef<T> coef;
-    coef.alpha = T(alpha);
-    coef.beta = T(beta);
-    coef.gamma = T(gamma);
-    coef.add_source = add_source ? 1 : 0;
+    coef.alpha = T(s.alpha);
+    coef.beta = T(s.beta);
+    coef.gamma = T(s.gamma);
+    coef.add_source = s.add_source ? 1 : 0;
     for (int i = 0; i < kMaxScales; ++i) {
-      coef.ck[i] = i < ns ? T(ck[s0 + i]) : T(0);
-      coef.half_c0[i] = (first && i < ns) ? T(0.5 * c0[s0 + i]) : T(0);
+      coef.ck[i] = i < ns ? T(s.ck[s0 + i]) : T(0);
+      coef.half_c0[i] = (s.first && i < ns) ? T(0.5 * s.c0[s0 + i]) : T(0);
     }
-    T* rs = r + int64_t(s0) * r_rows * nsig;
+    T* rs = s.r + int64_t(s0) * s.r_rows * nsig;
     if (s0 == 0) {
       int rc;
       if (vec_ok)
-        rc = launch_vec<T, MV>((nsig + MV - 1) / MV, first, true, rb, re, indptr, indices,
-                               vals, x_cur, x_old, x_new, rs, r_rows, nsig, ns, coef, st, out_perm);
+        rc = launch_vec<T, MV>((nsig + MV - 1) / MV, s.first, true, rb, re, s.indptr, s.indices,
+                               s.vals, s.x_cur, s.x_old, s.x_new, rs, s.r_rows, nsig, ns, coef, st,
+                               s.out_perm);
       else
-        rc = launch_vec<T, 1>(nsig, first, true, rb, re, indptr, indices, vals, x_cur,
-                              x_old, x_new, rs, r_rows, nsig, ns, coef, st, out_perm);
+        rc = launch_vec<T, 1>(nsig, s.first, true, rb, re, s.indptr, s.indices, s.vals, s.x_cur,
+                              s.x_old, s.x_new, rs, s.r_rows, nsig, ns, coef, st, s.out_perm);
       if (rc != GSP_OK) return rc;
     } else {
       // remaining scales of a wide bank: r_i (+)= c_ik * x_new, no second SpMM
@@ -260,49 +238,55 @@ int cheby_step(bool first, int64_t rb, int64_t re, const int32_t* indptr,
       if (count > 0) {
         const int blocks = (int)std::min<int64_t>(ceil_div(count, 256), int64_t(sm_count()) * 16);
         cheby_axpy_scales<T><<<blocks, 256, 0, st>>>(
-            count, x_new + rb * nsig, rs + rb * nsig, r_rows * nsig, ns, coef, first,
-            x_cur + rb * nsig);
+            count, s.x_new + rb * nsig, rs + rb * nsig, s.r_rows * nsig, ns, coef, s.first,
+            s.x_cur + rb * nsig);
         GSP_LAUNCH_CHECK("cheby_axpy_scales");
       }
     }
-    if (nscales == 0) break;
+    if (s.nscales == 0) break;
   }
   return GSP_OK;
 }
 
 template <typename T>
-static int cheby_step_planned(const gsp_tile_plan* plan, int64_t nnz, bool first, int64_t rb,
-                              int64_t re, const int32_t* indptr, const int32_t* indices,
-                              const T* vals, const T* x_cur, const T* x_old, T* x_new, T* r,
-                              int64_t r_rows, int nsig, int nscales, const double* ck,
-                              const double* c0, double alpha, double beta, double gamma,
-                              cudaStream_t st, bool add_source = false, bool reverse = false) {
-  return cheby_step<T>(first, rb, re, indptr, indices, vals, x_cur, x_old, x_new, r, r_rows, nsig,
-                       nscales, ck, c0, alpha, beta, gamma, st, add_source);
-}
-
-// float32 with a tile plan: TMA-tiled kernel on the full tiles of [rb, re), the
-// row-group kernel on the remaining (< rows_per_tile) rows.
-template <>
-int cheby_step_planned<float>(const gsp_tile_plan* plan, int64_t nnz, bool first, int64_t rb,
-                              int64_t re, const int32_t* indptr, const int32_t* indices,
-                              const float* vals, const float* x_cur, const float* x_old,
-                              float* x_new, float* r, int64_t r_rows, int nsig, int nscales,
-                              const double* ck, const double* c0, double alpha, double beta,
-                              double gamma, cudaStream_t st, bool add_source, bool reverse) {
-  const bool tiled = plan && plan->rows_per_tile > 0 && rb % 4 == 0 && nscales <= kMaxScales &&
-                     aligned16(indptr) && aligned16(indices) && aligned16(vals) &&
-                     aligned16(x_cur) && aligned16(x_new) && aligned16(r) &&
-                     (first || aligned16(x_old));
+int run_step(const Step<T>& s, int64_t rb, int64_t re, const gsp_tile_plan* plan,
+             const gsp_halo_fusion* halo, cudaStream_t st) {
+  const bool tiled = tiled_step_applies(s, rb, plan);
+  if (halo && !tiled)
+    return fail(GSP_ERR_UNSUPPORTED, "fused halo step: the tiled kernel does not apply (it needs "
+                "a tile plan, at most 16 filters and 16-byte aligned blocks)");
   int64_t done = 0;
-  if (tiled) {
-    int rc = cheby_step_tiled_f32(first, rb, re, nnz, indptr, indices, vals, x_cur, x_old, x_new, r,
-                                  r_rows, nsig, nscales, ck, c0, alpha, beta, gamma, *plan, nullptr,
-                                  &done, st, add_source, reverse);
-    if (rc != GSP_OK) return rc;
+  if constexpr (std::is_same<T, float>::value) {
+    if (halo) {
+      // (1) The boundary ("front") tiles -- those holding rows that read halo columns or that some
+      // neighbour needs -- with the halo-capable instantiation: wait for the neighbours' flags,
+      // coherent gathers, peer stores of the new boundary rows, publish.  (2) The interior tiles
+      // with the plain instantiation.  One kernel for both is slower per step (DESIGN.md section
+      // 5): under the 60-register cap ptxas spills the boundary code's state inside the interior
+      // gather loop.  The front launch is a few dozen tiles and publishes before the interior
+      // tiles run, so the neighbours' next front launch finds the flag set.
+      GSP_REQUIRE(rb == 0, "fused halo step needs the whole row block");
+      const int64_t R = plan->rows_per_tile;
+      const int64_t front = ceil_div(std::max<int64_t>(halo->publish ? halo->n_push_rows : 0,
+                                                       halo->n_boundary_rows), R) * R;
+      GSP_REQUIRE(front <= (re / R) * R, "boundary rows must lie inside the full tiles");
+      if (front > 0) {
+        Step<float> fs = s;
+        fs.reverse = false;
+        int rc = cheby_step_tiled_f32(fs, 0, front, *plan, halo, &done, st);
+        if (rc != GSP_OK) return rc;
+        GSP_REQUIRE(done == front, "front tiles must be whole tiles");
+      }
+    }
+    if (tiled) {
+      int64_t interior = 0;
+      int rc = cheby_step_tiled_f32(s, rb + done, re, *plan, nullptr, &interior, st);
+      if (rc != GSP_OK) return rc;
+      done += interior;
+    }
   }
-  return cheby_step<float>(first, rb + done, re, indptr, indices, vals, x_cur, x_old, x_new, r,
-                           r_rows, nsig, nscales, ck, c0, alpha, beta, gamma, st, add_source);
+  // the < rows_per_tile remainder (interior rows by the fused-step condition), or every row
+  return cheby_step<T>(s, rb + done, re, st);
 }
 
 // Full operator (approximations.py:58-114): K = m-1 fused steps on `stream`.
@@ -317,32 +301,24 @@ int cheby_op(int64_t n, int64_t nnz, const int32_t* indptr, const int32_t* indic
   double ck[1024], c0[1024];
   GSP_REQUIRE(nscales <= 1024, "at most 1024 filters per call");
   T* buf[2] = {work, work + n * int64_t(nsig)};
+  Step<T> s{nnz, indptr, indices, vals};
+  s.r = r;
+  s.r_rows = n;
+  s.nsig = nsig;
   const T* t_old = x;
   const T* t_cur = x;
   for (int k = 1; k < m; ++k) {
-    for (int i = 0; i < nscales; ++i) {
-      ck[i] = coeffs[int64_t(i) * m + k];
-      c0[i] = coeffs[int64_t(i) * m];
-    }
-    int rc;
-    if (k == 1) {
-      // T_1 = (L x - a x)/a = (2/lmax) L x - x ; r_i = c_i0/2 T_0 + c_i1 T_1
-      rc = cheby_step_planned<T>(plan, nnz, true, 0, n, indptr, indices, vals, x, nullptr, buf[0],
-                                 r, n, nsig, nscales, ck, c0, 2.0 / lmax, -1.0, 0.0, st);
-      t_cur = buf[0];
-    } else {
-      // T_k = (4/lmax) L T_{k-1} - 2 T_{k-1} - T_{k-2}, written over T_{k-2}
-      // (row-local) except for k == 2 where T_0 is the caller's input.
-      T* dst = (k == 2) ? buf[1] : const_cast<T*>(t_old);
-      // odd steps walk the tiles backwards: the lines of T_{k-1} and r that the previous
-      // step wrote last are still in L2 and are the first ones this step reads
-      rc = cheby_step_planned<T>(plan, nnz, false, 0, n, indptr, indices, vals, t_cur, t_old, dst,
-                                 r, n, nsig, nscales, ck, c0, 4.0 / lmax, -2.0, -1.0, st, false,
-                                 (k & 1) == 0);
-      t_old = t_cur;
-      t_cur = dst;
-    }
+    forward_coefs(s, k, m, nscales, lmax, coeffs, ck, c0);
+    // T_1 into buf[0]; T_k written over T_{k-2} (row-local) except for k == 2, where T_0 is the
+    // caller's input
+    T* dst = k == 1 ? buf[0] : (k == 2 ? buf[1] : const_cast<T*>(t_old));
+    s.x_cur = t_cur;
+    s.x_old = k == 1 ? nullptr : t_old;
+    s.x_new = dst;
+    int rc = run_step<T>(s, 0, n, plan, nullptr, st);
     if (rc != GSP_OK) return rc;
+    t_old = t_cur;
+    t_cur = dst;
   }
   return GSP_OK;
 }
@@ -379,29 +355,21 @@ int cheby_clenshaw(int64_t n, int64_t nnz, const int32_t* indptr, const int32_t*
   GSP_REQUIRE(lmax > 0 && lmax == lmax, "lmax must be positive");
   if (n == 0) return GSP_OK;
   const int K = m - 1;
-  const double a2 = 4.0 / lmax;                  // 2 Lt = a2 L - 2 I
   T* buf[2] = {work, work + n * int64_t(nsig)};
-  T* xs = const_cast<T*>(src);                   // read-only source blocks
-  double ck[kMaxScales], zero[kMaxScales];
-  for (int i = 0; i < kMaxScales; ++i) zero[i] = 0;
-  auto coef_col = [&](int k, double scale) {
-    for (int i = 0; i < nsrc; ++i) ck[i] = scale * c[int64_t(i) * m + k];
-  };
-  const T* b_cur;
+  double ck[kMaxScales];
+  Step<T> s{nnz, indptr, indices, vals};
+  s.r_rows = n;
+  s.nsig = nsig;
+  const T* b_cur = buf[0];
   const T* b_old = nullptr;
   int k_next;
   if (nsrc == 1) {
-    if (K == 1) {                                // out = c0/2 x + c1 Lt x
-      return cheby_step_planned<T>(plan, nnz, true, 0, n, indptr, indices, vals, src, nullptr,
-                                   out, out, n, nsig, 0, zero, zero, c[1] * 2.0 / lmax,
-                                   0.5 * c[0] - c[1], 0.0, st);
-    }
-    // b_{K-1} = c_{K-1} x + 2 Lt (c_K x): b_K = c_K x is never materialised
-    int rc = cheby_step_planned<T>(plan, nnz, true, 0, n, indptr, indices, vals, src, nullptr,
-                                   buf[0], buf[0], n, nsig, 0, zero, zero, c[K] * a2,
-                                   c[K - 1] - 2.0 * c[K], 0.0, st);
-    if (rc != GSP_OK) return rc;
-    b_cur = buf[0];
+    // b_{K-1} from x (with K == 1: out)
+    clenshaw_coefs(s, K - 1, m, 1, lmax, c, ck);
+    s.x_cur = src;
+    s.x_new = s.r = K == 1 ? out : buf[0];
+    int rc = run_step<T>(s, 0, n, plan, nullptr, st);
+    if (rc != GSP_OK || K == 1) return rc;
     k_next = K - 2;
   } else {
     // b_K = S_K by one combine pass
@@ -412,27 +380,16 @@ int cheby_clenshaw(int64_t n, int64_t nnz, const int32_t* indptr, const int32_t*
     const int blocks = (int)std::min<int64_t>(ceil_div(count, 256), int64_t(sm_count()) * 16);
     combine_sources<T><<<blocks, 256, 0, st>>>(count, src, nsrc, coef, buf[0]);
     GSP_LAUNCH_CHECK("combine_sources");
-    b_cur = buf[0];
     k_next = K - 1;
   }
+  s.r = const_cast<T*>(src);                      // read-only source blocks
   for (int k = k_next; k >= 0; --k) {
-    const bool last = k == 0;
-    // middle: b_k = a2 L b_{k+1} - 2 b_{k+1} - b_{k+2} + S_k
-    // last  : out = (a2/2) L b_1 - b_1 - b_2 + S_0/2
-    const double alpha = last ? 0.5 * a2 : a2, beta = last ? -1.0 : -2.0;
-    double gamma = -1.0;
-    coef_col(k, last ? 0.5 : 1.0);
-    const T* old = b_old;
-    if (!old) {
-      // no b_{k+2} buffer yet: it is c_K x (nsrc == 1, folded into the source term) or 0
-      if (nsrc == 1) ck[0] -= c[K];
-      gamma = 0.0;
-      old = b_cur;                                // any valid block, multiplied by 0
-    }
-    T* dst = last ? out : (b_old ? const_cast<T*>(b_old) : buf[1]);
-    int rc = cheby_step_planned<T>(plan, nnz, false, 0, n, indptr, indices, vals, b_cur, old, dst,
-                                   xs, n, nsig, nsrc, ck, zero, alpha, beta, gamma, st, true,
-                               (k & 1) == 0);
+    clenshaw_coefs(s, k, m, nsrc, lmax, c, ck);
+    T* dst = k == 0 ? out : (b_old ? const_cast<T*>(b_old) : buf[1]);
+    s.x_cur = b_cur;
+    s.x_old = b_old ? b_old : b_cur;              // no b_{k+2} yet: any valid block, times gamma = 0
+    s.x_new = dst;
+    int rc = run_step<T>(s, 0, n, plan, nullptr, st);
     if (rc != GSP_OK) return rc;
     b_old = b_cur;
     b_cur = dst;
@@ -446,19 +403,45 @@ template <typename T>
 int spmm_plain(int64_t n, const int32_t* indptr, const int32_t* indices, const T* vals,
                const T* x, int nsig, T* y, cudaStream_t st) {
   // x_new = 1 * (A x) + 0 * x ; FIRST form with nscales = 0 touches no r
-  double none = 0;
-  return cheby_step<T>(true, 0, n, indptr, indices, vals, x, nullptr, y, y, n, nsig, 0, &none,
-                       &none, 1.0, 0.0, 0.0, st);
+  Step<T> s{0, indptr, indices, vals};
+  s.x_cur = x;
+  s.x_new = s.r = y;
+  s.r_rows = n;
+  s.nsig = nsig;
+  s.first = true;
+  s.alpha = 1.0;
+  return run_step<T>(s, 0, n, nullptr, nullptr, st);
 }
 
-template int cheby_step<float>(bool, int64_t, int64_t, const int32_t*, const int32_t*,
-                               const float*, const float*, const float*, float*, float*,
-                               int64_t, int, int, const double*, const double*, double,
-                               double, double, cudaStream_t, bool, const int64_t*);
-template int cheby_step<double>(bool, int64_t, int64_t, const int32_t*, const int32_t*,
-                                const double*, const double*, const double*, double*, double*,
-                                int64_t, int, int, const double*, const double*, double,
-                                double, double, cudaStream_t, bool, const int64_t*);
+// a step as the C ABI passes it (gsp_cheby_step_*, gsp_cheby_step_halo_f32)
+template <typename T>
+static Step<T> abi_step(int first, int64_t nnz, const int32_t* indptr, const int32_t* indices,
+                        const T* data, const T* x_cur, const T* x_old, T* x_new, T* r,
+                        int64_t r_rows, int64_t nsig, int nscales, const double* ck,
+                        const double* c0, double alpha, double beta, double gamma) {
+  Step<T> s{nnz, indptr, indices, data};
+  s.x_cur = x_cur;
+  s.x_old = x_old;
+  s.x_new = x_new;
+  s.r = r;
+  s.r_rows = r_rows;
+  s.nsig = (int)nsig;
+  s.first = first != 0;
+  s.alpha = alpha;
+  s.beta = beta;
+  s.gamma = gamma;
+  s.nscales = nscales;
+  s.ck = ck;
+  s.c0 = c0;
+  return s;
+}
+
+template int cheby_step<float>(const Step<float>&, int64_t, int64_t, cudaStream_t);
+template int cheby_step<double>(const Step<double>&, int64_t, int64_t, cudaStream_t);
+template int run_step<float>(const Step<float>&, int64_t, int64_t, const gsp_tile_plan*,
+                             const gsp_halo_fusion*, cudaStream_t);
+template int run_step<double>(const Step<double>&, int64_t, int64_t, const gsp_tile_plan*,
+                              const gsp_halo_fusion*, cudaStream_t);
 
 }  // namespace gsp
 
@@ -481,10 +464,10 @@ extern "C" {
                            const double* c0_host, double alpha, double beta, double gamma,        \
                            const gsp_tile_plan* plan_host, void* stream) {                        \
     GSP_REQUIRE(nsig >= 1 && nsig <= (1 << 20), "nsig out of range");                             \
-    return gsp::cheby_step_planned<T>(plan_host, nnz, first != 0, row_begin, row_end, indptr,     \
-                                      indices, data, x_cur, x_old, x_new, r, r_rows, (int)nsig,   \
-                                      nscales, ck_host, c0_host, alpha, beta, gamma,              \
-                                      gsp::as_stream(stream));                                    \
+    return gsp::run_step<T>(gsp::abi_step<T>(first, nnz, indptr, indices, data, x_cur, x_old,      \
+                                             x_new, r, r_rows, nsig, nscales, ck_host, c0_host,   \
+                                             alpha, beta, gamma),                                 \
+                            row_begin, row_end, plan_host, nullptr, gsp::as_stream(stream));      \
   }                                                                                               \
   int gsp_cheby_clenshaw_##SUF(int64_t n, int64_t nnz, const int32_t* indptr,                     \
                                const int32_t* indices, const T* data, double lmax,                \
@@ -512,19 +495,13 @@ int gsp_cheby_step_halo_f32(int first, int64_t n_rows, int64_t nnz, const int32_
                             const double* c0_host, double alpha, double beta, double gamma,
                             int reverse, const gsp_tile_plan* plan_host,
                             const gsp_halo_fusion* halo_host, void* stream) {
-  if (!(plan_host && plan_host->rows_per_tile > 0 && halo_host))
-    return gsp::fail(GSP_ERR_UNSUPPORTED, "fused halo step needs a tile plan (%s)", "plan");
+  if (!halo_host) return gsp::fail(GSP_ERR_UNSUPPORTED, "fused halo step needs a halo description");
   GSP_REQUIRE(nscales <= gsp::kMaxScales, "too many filters for the fused step");
-  int64_t done = 0;
-  int rc = gsp::cheby_step_tiled_halo_f32(first != 0, n_rows, nnz, indptr, indices, data, x_cur,
-                                          x_old, x_new, r, r_rows, (int)nsig, nscales, ck_host,
-                                          c0_host, alpha, beta, gamma, *plan_host, *halo_host, &done,
-                                          gsp::as_stream(stream), false, reverse != 0, nullptr);
-  if (rc != GSP_OK) return rc;
-  // remainder rows (< rows_per_tile, interior by construction) with the row-group kernel
-  return gsp::cheby_step<float>(first != 0, done, n_rows, indptr, indices, data, x_cur, x_old,
-                                x_new, r, r_rows, (int)nsig, nscales, ck_host, c0_host, alpha,
-                                beta, gamma, gsp::as_stream(stream));
+  gsp::Step<float> s = gsp::abi_step<float>(first, nnz, indptr, indices, data, x_cur, x_old, x_new,
+                                            r, r_rows, nsig, nscales, ck_host, c0_host, alpha,
+                                            beta, gamma);
+  s.reverse = reverse != 0;
+  return gsp::run_step<float>(s, 0, n_rows, plan_host, halo_host, gsp::as_stream(stream));
 }
 
 }  // extern "C"

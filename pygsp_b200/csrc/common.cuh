@@ -54,17 +54,6 @@ inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 // number of SMs of the current device (cached per device)
 int sm_count();
 
-// ----- the fused recurrence step (csrc/cheby.cu), shared by Lanczos and the C ABI ---------
-// x_new = alpha (L x_cur) + beta x_cur + gamma x_old over rows [rb, re);
-//   add_source == false: r_i (+)= ck[i] x_new          (reference order, approximations.py:107-109)
-//   add_source == true : x_new += ck[0] * r[row, :]    (Clenshaw form, r is a read-only source)
-template <typename T>
-int cheby_step(bool first, int64_t rb, int64_t re, const int32_t* indptr, const int32_t* indices,
-               const T* vals, const T* x_cur, const T* x_old, T* x_new, T* r, int64_t r_rows,
-               int nsig, int nscales, const double* ck, const double* c0, double alpha,
-               double beta, double gamma, cudaStream_t st, bool add_source = false,
-               const int64_t* out_perm = nullptr);   // x_new row of local row i is out_perm[i]
-
 // indptr[1..n] (row sizes on entry) := their inclusive scan, indptr[0] = 0 -- csrc/graph.cu
 int scan_rows(int32_t* indptr, int64_t n, cudaStream_t st);
 

@@ -11,21 +11,11 @@
 //   base+1      entry barrier: nobody writes into a rank that is still in its previous call
 //   base+2      halo of T_0 (the input block) is in place
 //   base+2+s    halo of the block written by step s is in place, s = 1 .. K-1
-#include <type_traits>
 #include <vector>
 #include <cstdio>
-#include "common.cuh"
-#include "gspb200.h"
+#include "step.cuh"
 
 namespace gsp {
-
-int cheby_step_tiled_f32(bool first, int64_t rb, int64_t re, int64_t nnz, const int32_t* indptr,
-                         const int32_t* indices, const float* vals, const float* x_cur,
-                         const float* x_old, float* x_new, float* r, int64_t r_rows, int nsig,
-                         int nscales, const double* ck, const double* c0, double alpha, double beta,
-                         double gamma, const gsp_tile_plan& plan, const gsp_halo_fusion* halo,
-                         int64_t* rows_done, cudaStream_t st, bool add_source, bool reverse,
-                         const int64_t* out_perm);
 
 template <typename T> struct DistTraits;
 template <> struct DistTraits<float> {
@@ -47,18 +37,16 @@ template <> struct DistTraits<double> {
   }
 };
 
-// One step on the whole local block.  Fused form (float32 + tile plan): wait, push and publish
-// happen inside the step kernel; otherwise wait kernel -> step -> push kernel.
+// One step on the whole local block.  Fused form (the exchange fusable and the tiled kernel taking
+// the step): wait, push and publish happen inside the step kernel; otherwise wait kernel -> step ->
+// push kernel.  new_buf: the window block s.x_new points into (-1: the caller's r, not pushed).
 template <typename T>
-static int dist_step(const gsp_dist_plan* p, const gsp_tile_plan* tile, bool fused, bool first,
-                     const T* x_cur, const T* x_old, T* x_new, int new_buf, T* r, int64_t r_rows,
-                     int nsig, int nscales, const double* ck, const double* c0, double alpha,
-                     double beta, double gamma, bool add_source, bool reverse, uint64_t wait_value,
-                     uint64_t publish_value, bool publish, void* stream,
-                     const int64_t* out_perm = nullptr) {
+static int dist_step(const gsp_dist_plan* p, const gsp_tile_plan* tile, bool fusable,
+                     const Step<T>& s, int new_buf, uint64_t wait_value, uint64_t publish_value,
+                     bool publish, void* stream) {
   cudaStream_t st = as_stream(stream);
   const int64_t n = p->n_local;
-  if (fused) {
+  if (fusable && tiled_step_applies(s, 0, tile)) {
     gsp_halo_fusion h;
     memset(&h, 0, sizeof(h));
     h.n_push_rows = publish ? p->n_push_rows : 0;
@@ -77,60 +65,14 @@ static int dist_step(const gsp_dist_plan* p, const gsp_tile_plan* tile, bool fus
     h.n_boundary_rows = p->n_boundary_rows;
     h.n_owned = n;
     h.publish = publish ? 1 : 0;
-    // Two launches on the same stream.  (1) The boundary ("front") tiles with the
-    // halo-capable instantiation: wait for the neighbours' flags, coherent gathers, peer
-    // stores of the new boundary rows, publish.  (2) All interior tiles with the plain
-    // instantiation.  One kernel for both is slower per step: the boundary code's registers
-    // spill inside the interior tiles' gather loop (ptxas, 60-register cap); the front
-    // launch is a few dozen tiles and publishes before the interior runs.
-    const int R = tile->rows_per_tile;
-    const int64_t front_rows =
-        ceil_div(std::max<int64_t>(publish ? p->n_push_rows : 0, p->n_boundary_rows), (int64_t)R) * R;
-    int64_t done = 0, done_front = 0;
-    int rc = GSP_OK;
-    if (front_rows > 0) {
-      rc = cheby_step_tiled_f32(first, 0, front_rows, p->nnz, p->indptr, p->indices,
-                                reinterpret_cast<const float*>(p->data),
-                                reinterpret_cast<const float*>(x_cur),
-                                reinterpret_cast<const float*>(x_old),
-                                reinterpret_cast<float*>(x_new), reinterpret_cast<float*>(r), r_rows,
-                                nsig, nscales, ck, c0, alpha, beta, gamma, *tile, &h, &done_front, st,
-                                add_source, false, out_perm);
-      if (rc != GSP_OK) return rc;
-      GSP_REQUIRE(done_front == front_rows, "front tiles must be whole tiles");
-    }
-    rc = cheby_step_tiled_f32(first, front_rows, n, p->nnz, p->indptr, p->indices,
-                              reinterpret_cast<const float*>(p->data),
-                              reinterpret_cast<const float*>(x_cur),
-                              reinterpret_cast<const float*>(x_old), reinterpret_cast<float*>(x_new),
-                              reinterpret_cast<float*>(r), r_rows, nsig, nscales, ck, c0, alpha, beta,
-                              gamma, *tile, nullptr, &done, st, add_source, reverse, out_perm);
-    if (rc != GSP_OK) return rc;
-    done += front_rows;
-    // remainder rows (< rows_per_tile; interior by the fused-form condition)
-    return cheby_step<T>(first, done, n, p->indptr, p->indices, static_cast<const T*>(p->data), x_cur,
-                         x_old, x_new, r, r_rows, nsig, nscales, ck, c0, alpha, beta, gamma, st,
-                         add_source, out_perm);
+    return run_step<T>(s, 0, n, tile, &h, st);
   }
   int rc = gsp_halo_wait(p->flags, p->neighbor_ids, p->n_neighbors, wait_value, stream);
   if (rc != GSP_OK) return rc;
-  int64_t done = 0;
-  if (std::is_same<T, float>::value && tile && tile->rows_per_tile > 0) {
-    // the TMA-tiled kernel without the fused exchange (the halo is complete: the wait kernel
-    // ran), then the row-group kernel on the < rows_per_tile remainder
-    rc = cheby_step_tiled_f32(first, 0, n, p->nnz, p->indptr, p->indices,
-                              reinterpret_cast<const float*>(p->data),
-                              reinterpret_cast<const float*>(x_cur),
-                              reinterpret_cast<const float*>(x_old), reinterpret_cast<float*>(x_new),
-                              reinterpret_cast<float*>(r), r_rows, nsig, nscales, ck, c0, alpha, beta,
-                              gamma, *tile, nullptr, &done, st, add_source, reverse, out_perm);
-    if (rc != GSP_OK) return rc;
-  }
-  rc = cheby_step<T>(first, done, n, p->indptr, p->indices, static_cast<const T*>(p->data), x_cur,
-                     x_old, x_new, r, r_rows, nsig, nscales, ck, c0, alpha, beta, gamma, st,
-                     add_source, out_perm);
+  // the halo is complete (the wait kernel ran): a step without the fused exchange
+  rc = run_step<T>(s, 0, n, tile, nullptr, st);
   if (rc != GSP_OK) return rc;
-  if (publish) return DistTraits<T>::push(p, p->n_send, new_buf, publish_value, nsig, stream);
+  if (publish) return DistTraits<T>::push(p, p->n_send, new_buf, publish_value, s.nsig, stream);
   return GSP_OK;
 }
 
@@ -180,9 +122,10 @@ int cheby_op_dist(const gsp_dist_plan* p, const gsp_tile_plan* tile, double lmax
   const uint64_t base = *seq;
   *seq = base + uint64_t(m) + 2;
   T* buf[3] = {static_cast<T*>(p->buf[0]), static_cast<T*>(p->buf[1]), static_cast<T*>(p->buf[2])};
-  const bool tiled = std::is_same<T, float>::value && tile && tile->rows_per_tile > 0;
-  const bool fused =
-      tiled && !p->separate_exchange && p->n_neighbors >= 1 && p->n_neighbors <= 32 &&
+  // a step fuses the exchange when this holds and the tiled kernel takes it (dist_step)
+  const bool fusable =
+      tile && tile->rows_per_tile > 0 && !p->separate_exchange && p->n_neighbors >= 1 &&
+      p->n_neighbors <= 32 &&
       std::max(p->n_push_rows, p->n_boundary_rows) <= (n / tile->rows_per_tile) * tile->rows_per_tile;
   if (clenshaw && (nscales != 1 || K < 2 || !buf[2])) clenshaw = 0;
 
@@ -204,8 +147,10 @@ int cheby_op_dist(const gsp_dist_plan* p, const gsp_tile_plan* tile, double lmax
   if (rc != GSP_OK) return rc;
   trace.mark();
 
-  double ck[16], c0[16], zero[16];
-  for (int i = 0; i < 16; ++i) zero[i] = 0;
+  double ck[16], c0[16];
+  Step<T> s{p->nnz, p->indptr, p->indices, static_cast<const T*>(p->data)};
+  s.r_rows = n;
+  s.nsig = nsig;
   if (!clenshaw) {
     // forward recurrence, reference order (approximations.py:99-112).  With a row
     // permutation the accumulators live in local order in stream-ordered scratch and are
@@ -214,17 +159,14 @@ int cheby_op_dist(const gsp_dist_plan* p, const gsp_tile_plan* tile, double lmax
     if (perm && n > 0) {
       GSP_CUDA(cudaMallocAsync((void**)&r, sizeof(T) * size_t(nscales) * n * nsig, st));
     }
+    s.r = r;
     int cur = 0, old = 1;
     for (int k = 1; k <= K; ++k) {
-      for (int i = 0; i < nscales; ++i) {
-        ck[i] = c[int64_t(i) * m + k];
-        c0[i] = c[int64_t(i) * m];
-      }
-      const bool first = k == 1;
-      rc = dist_step<T>(p, tile, fused, first, buf[cur], first ? nullptr : buf[old], buf[old], old, r,
-                        n, nsig, nscales, ck, c0, first ? 2.0 / lmax : 4.0 / lmax,
-                        first ? -1.0 : -2.0, first ? 0.0 : -1.0, false, (k & 1) == 0,
-                        base + 1 + k, base + 2 + k, k < K, stream);
+      forward_coefs(s, k, m, nscales, lmax, c, ck, c0);
+      s.x_cur = buf[cur];
+      s.x_old = s.first ? nullptr : buf[old];
+      s.x_new = buf[old];
+      rc = dist_step<T>(p, tile, fusable, s, old, base + 1 + k, base + 2 + k, k < K, stream);
       if (rc != GSP_OK) { if (r != r_out) cudaFreeAsync(r, st); return rc; }
       trace.mark();
       std::swap(cur, old);
@@ -239,29 +181,24 @@ int cheby_op_dist(const gsp_dist_plan* p, const gsp_tile_plan* tile, double lmax
   }
   // Clenshaw, single filter (see cheby_clenshaw in cheby.cu): buf[0] keeps x (the source),
   // b_{K-1} -> buf[1], b_{K-2} -> buf[2], b_{K-3} -> buf[1], ...; the last step writes r.
-  const double a2 = 4.0 / lmax;
-  rc = dist_step<T>(p, tile, fused, true, buf[0], nullptr, buf[1], 1, buf[1], n, nsig, 0, zero, zero,
-                    c[K] * a2, c[K - 1] - 2.0 * c[K], 0.0, false, false, base + 2, base + 3, true,
-                    stream);
+  clenshaw_coefs(s, K - 1, m, 1, lmax, c, ck);
+  s.x_cur = buf[0];
+  s.x_new = s.r = buf[1];
+  rc = dist_step<T>(p, tile, fusable, s, 1, base + 2, base + 3, true, stream);
   if (rc != GSP_OK) return rc;
   trace.mark();
+  s.r = buf[0];
   int cur = 1, old = -1, step = 1;
   for (int k = K - 2; k >= 0; --k) {
     ++step;
     const bool last = k == 0;
-    double gamma = -1.0;
-    ck[0] = (last ? 0.5 : 1.0) * c[k];
-    int old_buf = old;
-    if (old < 0) {                       // b_{K} = c_K x is folded into the source term
-      ck[0] -= c[K];
-      gamma = 0.0;
-      old_buf = cur;
-    }
+    clenshaw_coefs(s, k, m, 1, lmax, c, ck);
     const int dst = last ? -1 : (old >= 0 ? old : 2);
-    T* x_new = last ? r : buf[dst];
-    rc = dist_step<T>(p, tile, fused, false, buf[cur], buf[old_buf], x_new, dst, buf[0], n, nsig, 1,
-                      ck, zero, last ? 0.5 * a2 : a2, last ? -1.0 : -2.0, gamma, true, (k & 1) == 0,
-                      base + 1 + step, base + 2 + step, !last, stream, last ? perm : nullptr);
+    s.x_cur = buf[cur];
+    s.x_old = buf[old >= 0 ? old : cur];   // no b_{k+2} yet: any valid block, times gamma = 0
+    s.x_new = last ? r : buf[dst];
+    s.out_perm = last ? perm : nullptr;
+    rc = dist_step<T>(p, tile, fusable, s, dst, base + 1 + step, base + 2 + step, !last, stream);
     if (rc != GSP_OK) return rc;
     trace.mark();
     old = cur;

@@ -19,18 +19,9 @@
 // The one-hot Y is never formed: label[row] is the class of a labelled vertex, -1 otherwise.
 #include <math.h>
 
-#include "common.cuh"
-#include "gspb200.h"
+#include "step.cuh"
 
 namespace gsp {
-
-int cheby_step_tiled_f32(bool first, int64_t rb, int64_t re, int64_t nnz, const int32_t* indptr,
-                         const int32_t* indices, const float* vals, const float* x_cur,
-                         const float* x_old, float* x_new, float* r, int64_t r_rows, int nsig,
-                         int nscales, const double* ck, const double* c0, double alpha, double beta,
-                         double gamma, const gsp_tile_plan& plan, const gsp_halo_fusion* halo,
-                         int64_t* rows_done, cudaStream_t st, bool add_source = false,
-                         bool reverse = false, const int64_t* out_perm = nullptr);
 
 constexpr int kFbThreads = 256;
 constexpr int kFbMaxBlocks = 1024;
@@ -206,34 +197,6 @@ fb_row_kernel(int64_t n, int C, int w, const int32_t* __restrict__ label,
   }
 }
 
-// L X: the tiled float32 step on the full tiles where a plan applies, the row-group step on
-// the rest (as gsp_cheby_step_f32 does)
-template <typename T>
-static int apply_laplacian(int64_t n, int64_t nnz, const int32_t* indptr, const int32_t* indices,
-                           const T* data, const T* X, T* LX, int C, const gsp_tile_plan* plan,
-                           cudaStream_t st) {
-  const double zero = 0;
-  return cheby_step<T>(true, 0, n, indptr, indices, data, X, X, LX, LX, n, C, 0, &zero, &zero, 1.0,
-                       0.0, 0.0, st);
-}
-
-template <>
-int apply_laplacian<float>(int64_t n, int64_t nnz, const int32_t* indptr, const int32_t* indices,
-                           const float* data, const float* X, float* LX, int C,
-                           const gsp_tile_plan* plan, cudaStream_t st) {
-  const double zero = 0;
-  auto a16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
-  int64_t done = 0;
-  if (plan && plan->rows_per_tile > 0 && a16(indptr) && a16(indices) && a16(data) && a16(X) &&
-      a16(LX)) {
-    int rc = cheby_step_tiled_f32(true, 0, n, nnz, indptr, indices, data, X, X, LX, LX, n, C, 0,
-                                  &zero, &zero, 1.0, 0.0, 0.0, *plan, nullptr, &done, st);
-    if (rc != GSP_OK) return rc;
-  }
-  return cheby_step<float>(true, done, n, indptr, indices, data, X, X, LX, LX, n, C, 0, &zero,
-                           &zero, 1.0, 0.0, 0.0, st);
-}
-
 template <typename T, int V>
 static int launch_row(int blocks, int64_t n, int C, int w, const int32_t* label, const T* Xk,
                       const T* Xprev, const T* LXk, const T* LXprev, T* Xout, double tau,
@@ -271,6 +234,11 @@ int fb_simplex_run(int64_t n, int64_t nnz, const int32_t* indptr, const int32_t*
     fb_init_kernel<T><<<ib, kFbThreads, 0, st>>>(n, C, label, X2, scal);
     GSP_LAUNCH_CHECK("fb_init_kernel");
   }
+  Step<T> lap{nnz, indptr, indices, data};        // L X_k: the first form, alpha = 1, no r_i
+  lap.r_rows = n;
+  lap.nsig = C;
+  lap.first = true;
+  lap.alpha = 1.0;
   for (int it = it0; it < it1; ++it) {
     T* Xk = X2 + (it % 2) * nc;
     T* Xo = X2 + ((it + 1) % 2) * nc;
@@ -279,7 +247,9 @@ int fb_simplex_run(int64_t n, int64_t nnz, const int32_t* indptr, const int32_t*
     // iteration 0 has no x_{-1}: read x_0 in its place (beta = 0 there)
     const T* Xp = it == 0 ? Xk : Xo;
     const T* LXp = it == 0 ? LXk : LXo;
-    int rc = apply_laplacian<T>(n, nnz, indptr, indices, data, Xk, LXk, C, plan, st);
+    lap.x_cur = lap.x_old = Xk;
+    lap.x_new = lap.r = LXk;
+    int rc = run_step<T>(lap, 0, n, plan, nullptr, st);
     if (rc != GSP_OK) return rc;
     switch (V) {
       case 1: rc = launch_row<T, 1>(blocks, n, C, w, label, Xk, Xp, LXk, LXp, Xo, tau, step, it, stop, scal, st); break;
