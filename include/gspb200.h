@@ -448,7 +448,8 @@ int gsp_cheby_op_dist_f64(const gsp_dist_plan* plan_host, const gsp_tile_plan* t
  * gsp_grid2d_*: adjacency of pygsp/graphs/grid2d.py:40-89 (n1 x n2 grid, 4 neighbours, unit
  *     weights, row-major numbering) as canonical CSR; count writes indptr (n1*n2 + 1).
  * gsp_knn_grid: k nearest neighbours (self excluded) of n points in 2-D / 3-D by a
- *     uniform cell grid -- the scipy.spatial.KDTree query of nngraph.py:213-216.
+ *     uniform cell grid -- the scipy.spatial.KDTree query of nngraph.py:213-216 for the
+ *     Euclidean metric; other dimensions and metrics: gsp_knn_brute below.
  *     points (n, dim) double; lo/hi: bounding box, cells: grid resolution (host arrays
  *     of length dim); outputs (n, k) row-major, ascending distance, ties by index.
  * gsp_knn_to_csr_*: directed k-NN matrix W[i, nn] = exp(-d^2/sigma) as CSR with sorted
@@ -467,6 +468,48 @@ int gsp_knn_to_csr_f32(int64_t n, int k, const int32_t* nn_idx, const double* nn
 int gsp_knn_to_csr_f64(int64_t n, int k, const int32_t* nn_idx, const double* nn_dist,
                        double sigma, int32_t* indptr, int32_t* indices, double* data,
                        void* stream);
+
+/* ----------------------------------------------------- neighbour search, any dimension ---
+ * Exhaustive search over n points of dimension d >= 1 (points (n, d) row-major double), in the
+ * Minkowski metric of order p: p = 1 (manhattan), 2 (euclidean), INFINITY (max_dist) or any
+ * p >= 1 (minkowski: (sum |x_i - y_i|^p)^(1/p)); nngraph.py:162-167's dist_translation.  The
+ * difference is accumulated in dimension order, in double, and the root is taken once (as
+ * cKDTree).  Self is excluded by index, never by position.  csrc/neighbors.cu.
+ * gsp_knn_brute: nngraph.py:213-216, KDTree(X).query(X, k + 1, p) without the self column, for
+ *     any d.  1 <= k <= 32, k < n.  Outputs (n, k) like gsp_knn_grid: ascending (distance, id),
+ *     independent of the launch configuration.
+ * gsp_radius_count / gsp_radius_fill_f64: nngraph.py:228-283, query_ball_point(r = epsilon, p)
+ *     and the j != i filter: row i = {j != i : dist(x_i, x_j) <= epsilon}.  count writes indptr
+ *     (n + 1) and the number of entries to *nnz (device int64); indptr is meaningful only when
+ *     *nnz < 2^31, which the caller checks before allocating.  fill writes the columns (sorted,
+ *     bit-identical from run to run) and their distances (double).
+ * gsp_csr_symmetrize_count_* / _fill_*: utils.py:244-277 symmetrize(W, method) for mode
+ *     0 'maximum' (W - W o [W^T > W] + W^T o [W^T > W]), 1 'fill' (W + ((A + A^T) - A) o W^T,
+ *     A = W > 0, then 'average'), 2 'tril' and 3 'triu' (one triangle, then 'maximum').  A is W,
+ *     B = W^T (gsp_csr_transpose_*); exact zeros are dropped.  'average' is gsp_csr_average_*.
+ * gsp_gauss_weights_*: w = exp(-d^2 / sigma) for nnz distances (nngraph.py:276-281).
+ */
+int gsp_knn_brute(int64_t n, int d, const double* points, int k, double p, int32_t* nn_idx,
+                  double* nn_dist, void* stream);
+int gsp_radius_count(int64_t n, int d, const double* points, double epsilon, double p,
+                     int32_t* indptr, int64_t* nnz, void* stream);
+int gsp_radius_fill_f64(int64_t n, int d, const double* points, double epsilon, double p,
+                        const int32_t* indptr, int32_t* indices, double* dist, void* stream);
+
+#define GSPB200_DECLARE_NEIGHBOR_API(SUF, T)                                                     \
+  int gsp_csr_symmetrize_count_##SUF(int64_t n, int mode, const int32_t* a_indptr,               \
+                                     const int32_t* a_indices, const T* a_data,                  \
+                                     const int32_t* b_indptr, const int32_t* b_indices,          \
+                                     const T* b_data, int32_t* s_indptr, void* stream);          \
+  int gsp_csr_symmetrize_fill_##SUF(int64_t n, int mode, const int32_t* a_indptr,                \
+                                    const int32_t* a_indices, const T* a_data,                   \
+                                    const int32_t* b_indptr, const int32_t* b_indices,           \
+                                    const T* b_data, const int32_t* s_indptr,                    \
+                                    int32_t* s_indices, T* s_data, void* stream);                \
+  int gsp_gauss_weights_##SUF(int64_t nnz, const double* dist, double sigma, T* w, void* stream);
+
+GSPB200_DECLARE_NEIGHBOR_API(f32, float)
+GSPB200_DECLARE_NEIGHBOR_API(f64, double)
 
 #define GSPB200_DECLARE_GRAPH_API(SUF, T)                                                        \
   int gsp_csr_inspect_##SUF(int64_t n, const int32_t* indptr, const int32_t* indices,            \

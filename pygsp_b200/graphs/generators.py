@@ -6,6 +6,7 @@ construction is vectorised -- the reference's per-vertex Python loops
 (nngraph.py:221-226) make it unusable beyond ~1e6 vertices.  They are input
 fabrication for the filtering path, not part of the timed hot path.
 """
+import ctypes
 import os
 
 import numpy as np
@@ -14,7 +15,7 @@ from scipy import sparse, spatial
 from .. import _native as nat
 from .. import utils
 from .csr import DeviceCSR
-from .graph import Graph, _torch_dtype, symmetrize_average_device
+from .graph import Graph, _torch_dtype, symmetrize_average_device, symmetrize_device
 
 _DATA = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "data")
 
@@ -123,17 +124,39 @@ def grid2d_adjacency_device(N1, N2, dtype=None, device=None):
     return DeviceCSR(indptr, indices, data, (n, n))
 
 
-def knn_device(points, k, device=None, points_per_cell=3.0):
-    """k nearest neighbours of every point (self excluded) on the GPU.
+def _device_points(points, dev):
+    torch = nat.require_cuda()
+    return torch.as_tensor(np.asarray(points, dtype=np.float64) if not torch.is_tensor(points)
+                           else points).to(device=dev, dtype=torch.float64).contiguous()
 
-    Stands in for ``scipy.spatial.KDTree(X).query(X, k + 1)`` (nngraph.py:213-216):
-    returns (nn, dist), both (N, k) CUDA tensors, ascending distance.  2-D / 3-D, k <= 32.
+
+def _check_order(p):
+    p = float(p)
+    if not p >= 1:
+        raise ValueError("Only p-norms with 1<=p<=infinity permitted (p = {}).".format(p))
+    return p
+
+
+def knn_device(points, k, device=None, points_per_cell=3.0, p=2):
+    """k nearest neighbours of every point (self excluded by index) on the GPU.
+
+    Stands in for ``scipy.spatial.KDTree(X).query(X, k + 1, p=p)`` (nngraph.py:213-216):
+    returns (nn, dist), both (N, k) CUDA tensors, ascending (distance, id); k <= 32.  Euclidean
+    2-D / 3-D clouds are searched on a cell grid (``gsp_knn_grid``), every other dimension and
+    Minkowski order p >= 1 (inf included) exhaustively (``gsp_knn_brute``); both are exact.
     """
     torch = nat.require_cuda()
     dev = _device_of(device)
-    pts = torch.as_tensor(np.asarray(points, dtype=np.float64) if not torch.is_tensor(points)
-                          else points).to(device=dev, dtype=torch.float64).contiguous()
+    p = _check_order(p)
+    pts = _device_points(points, dev)
     n, dim = pts.shape
+    if p != 2 or dim not in (2, 3):
+        nn = torch.empty((n, k), dtype=torch.int32, device=dev)
+        dist = torch.empty((n, k), dtype=torch.float64, device=dev)
+        with torch.cuda.device(dev):
+            nat.call("gsp_knn_brute", nat.i64(n), nat.i32(dim), pts, nat.i32(k), nat.f64(p), nn,
+                     dist, nat.stream_ptr(dev))
+        return nn, dist
     lo = pts.min(dim=0).values.cpu().numpy().astype(np.float64)
     hi = pts.max(dim=0).values.cpu().numpy().astype(np.float64)
     span = np.maximum(hi - lo, 1e-300)
@@ -168,47 +191,304 @@ def knn_adjacency_device(points, k, sigma=None, dtype=None, device=None):
     return symmetrize_average_device(DeviceCSR(indptr, indices, data, (n, n))), sigma
 
 
-class NNGraph(Graph):
-    r"""k-nearest-neighbour graph of a point cloud with Gaussian weights.
+def radius_device(points, epsilon, p=2, device=None):
+    """Radius neighbourhoods of every point on the GPU: a (N, N) DeviceCSR of float64 distances.
 
-    ``w_ij = exp(-d_ij^2 / sigma)`` for the k nearest neighbours j of i, sigma =
-    mean neighbour distance, then ``W <- (W + W^T)/2`` -- the 'knn' branch of
-    pygsp/graphs/nngraphs/nngraph.py:147-226,289-297 with its default
-    ``center`` / ``rescale`` preprocessing (:127-136).  ``backend='device'`` (default for
-    2-D / 3-D clouds, k <= 32) searches and assembles in HBM (csrc/generate.cu);
-    ``backend='host'`` uses scipy's cKDTree.  Both give the same adjacency.
+    Row i holds the j != i with ``dist(x_i, x_j) <= epsilon`` in the Minkowski metric of order p,
+    sorted by column -- ``KDTree(X).query_ball_point(X, r=epsilon, p=p)`` and the self filter of
+    nngraph.py:228-283.  The number of entries is read once; ``ValueError`` when it does not fit
+    int32 CSR offsets or the free device memory, before anything is allocated for them.
+    """
+    torch = nat.require_cuda()
+    dev = _device_of(device)
+    p = _check_order(p)
+    pts = _device_points(points, dev)
+    n, dim = pts.shape
+    indptr = torch.empty(n + 1, dtype=torch.int32, device=dev)
+    total = torch.zeros(1, dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):
+        nat.call("gsp_radius_count", nat.i64(n), nat.i32(dim), pts, nat.f64(epsilon), nat.f64(p),
+                 indptr, total, nat.stream_ptr(dev))
+        nnz = int(total.item())
+        if nnz >= 2 ** 31:
+            raise ValueError("the radius graph has %d entries: more than int32 CSR offsets hold "
+                             "(lower epsilon)" % nnz)
+        free = torch.cuda.mem_get_info(dev)[0]
+        if 12 * nnz > free:
+            raise ValueError("the radius graph has %d entries (%d bytes): more than the free "
+                             "device memory (%d bytes)" % (nnz, 12 * nnz, free))
+        indices = torch.empty(nnz, dtype=torch.int32, device=dev)
+        dist = torch.empty(nnz, dtype=torch.float64, device=dev)
+        nat.call("gsp_radius_fill_f64", nat.i64(n), nat.i32(dim), pts, nat.f64(epsilon),
+                 nat.f64(p), indptr, indices, dist, nat.stream_ptr(dev))
+    return DeviceCSR(indptr, indices, dist, (n, n))
+
+
+def _gauss_weights_device(D, sigma, dt):
+    """DeviceCSR of exp(-d^2 / sigma) on the structure of a distance matrix D."""
+    torch = nat.require_cuda()
+    w = torch.empty(D.nnz, dtype=dt, device=D.device)
+    with torch.cuda.device(D.device):
+        nat.call("gsp_gauss_weights_" + nat.suffix(dt), nat.i64(D.nnz), D.data, nat.f64(sigma), w,
+                 nat.stream_ptr(D.device))
+    return DeviceCSR(D.indptr, D.indices, w, D.shape)
+
+
+_DIST_ORDER = {"euclidean": 2.0, "manhattan": 1.0, "max_dist": np.inf}
+_SYMMETRIZE_TYPES = ("average", "maximum", "fill", "tril", "triu")
+_logger = utils.build_logger(__name__)
+
+
+def _minkowski_order(dist_type, order, use_flann):
+    """(p, renumbering) from NNGraph's dist_type and order.
+
+    ``order`` renumbers vertices (None, 'morton' or a permutation).  The reference uses it as
+    the Minkowski order instead (nngraph.py:162-167); a real scalar was never a renumbering, so
+    with dist_type='minkowski' a scalar is p.  Without one p is the reference's default 0, which
+    its scikit-learn branch (use_flann=True) turns into the Euclidean metric and KDTree refuses.
+    """
+    if dist_type not in ("euclidean", "manhattan", "max_dist", "minkowski"):
+        raise ValueError("Unknown dist_type {}.".format(dist_type))
+    if dist_type != "minkowski":
+        return _DIST_ORDER[dist_type], order
+    scalar = order is not None and np.ndim(order) == 0 and not isinstance(order, str)
+    p = float(order) if scalar else 0.0
+    if p <= 0 and use_flann:
+        p = 2.0
+    return _check_order(p), (None if scalar else order)
+
+
+def _host_knn(X, k, p):
+    D, NN = spatial.cKDTree(X).query(X, k=k + 1, p=p, workers=-1)
+    return D[:, 1:], NN[:, 1:]
+
+
+def _host_radius(X, epsilon, p):
+    """Rows of query_ball_point without self (sorted) and their distances, as COO arrays."""
+    lists = spatial.cKDTree(X).query_ball_point(X, r=epsilon, p=p, workers=-1,
+                                                return_sorted=True)
+    rows = np.repeat(np.arange(X.shape[0]), [len(nb) for nb in lists])
+    cols = np.concatenate([np.asarray(nb, dtype=np.int64) for nb in lists]) if len(lists) else \
+        np.zeros(0, dtype=np.int64)
+    keep = rows != cols
+    rows, cols = rows[keep], cols[keep]
+    diff = np.abs(X[rows] - X[cols])
+    if p == 2:
+        dist = np.sqrt(np.sum(diff * diff, axis=1))
+    elif p == 1:
+        dist = np.sum(diff, axis=1)
+    elif np.isinf(p):
+        dist = diff.max(axis=1) if diff.size else np.zeros(0)
+    else:
+        dist = np.sum(diff ** p, axis=1) ** (1.0 / p)
+    return rows, cols, dist
+
+
+class NNGraph(Graph):
+    r"""Nearest-neighbour graph of a point cloud with Gaussian weights.
+
+    pygsp/graphs/nngraphs/nngraph.py:92-299 with its ``center`` / ``rescale`` preprocessing
+    (:127-136).  ``NNtype='knn'``: the k nearest neighbours j of every i, sigma = mean of the
+    k neighbour distances; ``NNtype='radius'``: every j != i within ``epsilon``, sigma = mean of
+    those distances (``ValueError`` when there is none).  ``w_ij = exp(-d_ij^2 / sigma)`` for
+    every metric, then ``utils.symmetrize(W, symmetrize_type)``.  ``dist_type``: 'euclidean',
+    'manhattan', 'max_dist' or 'minkowski' (order p >= 1 given as ``order``, see
+    :func:`_minkowski_order`).  The search is always exact: ``use_flann`` is accepted and
+    changes nothing.
+
+    ``backend=None`` picks the device for k <= 32 (a cell grid for Euclidean k-NN of 2-D / 3-D
+    clouds, an exhaustive search otherwise; csrc/generate.cu, csrc/neighbors.cu) and scipy's
+    cKDTree on the host for larger k; ``'device'`` / ``'host'`` force the choice.  ``Xin`` may
+    be a CUDA tensor (the patch graphs build their features on the device).
     """
 
     def __init__(self, Xin, k=10, sigma=None, center=True, rescale=True, order=None,
-                 backend=None, **kwargs):
-        Xin = np.asarray(Xin, dtype=np.float64)
+                 backend=None, *, NNtype="knn", use_flann=False, epsilon=0.01,
+                 symmetrize_type="average", dist_type="euclidean", **kwargs):
+        if NNtype not in ("knn", "radius"):
+            raise ValueError("Unknown NNtype {}".format(NNtype))
+        if symmetrize_type not in _SYMMETRIZE_TYPES:
+            raise ValueError("Unknown symmetrization method {}.".format(symmetrize_type))
+        p, order = _minkowski_order(dist_type, order, use_flann)
+        if use_flann:
+            _logger.debug("use_flann: the neighbour search is exact, FLANN is not used")
+        self.NNtype, self.use_flann, self.epsilon = NNtype, use_flann, epsilon
+        self.symmetrize_type, self.dist_type = symmetrize_type, dist_type
+        self.center, self.rescale = center, rescale
+        on_device = _is_tensor(Xin)
+        if not on_device:
+            Xin = np.asarray(Xin, dtype=np.float64)
+        self.Xin = Xin
         N, d = Xin.shape
         if k >= N:
             raise ValueError("The number of neighbors (k={}) must be smaller than the number "
                              "of nodes ({}).".format(k, N))
-        X = Xin - Xin.mean(axis=0) if center else Xin.copy()
-        if rescale:
-            radius = 0.5 * np.linalg.norm(X.max(axis=0) - X.min(axis=0), 2)
-            X *= (np.power(N, 1.0 / float(min(d, 3))) / 10.0) / radius
-        if order == "morton":
-            X = X[morton_order(X)]
-        elif order is not None:
-            X = X[np.asarray(order)]
-        if backend is None:     # the device search covers 2-D / 3-D clouds and k <= 32
-            backend = "device" if (d in (2, 3) and k <= 32) else "host"
-        if backend == "device":                     # grid-hash k-NN + symmetrisation in HBM
-            W, sigma = knn_adjacency_device(X, k, sigma, kwargs.get("dtype"), kwargs.get("device"))
-            self.k, self.sigma = k, sigma
+        if on_device:
+            torch = nat.require_cuda()
+            X = Xin.to(torch.float64)
+            X = X - X.mean(dim=0) if center else X.clone()
+            if rescale:
+                span = X.max(dim=0).values - X.min(dim=0).values
+                radius = 0.5 * float(torch.linalg.vector_norm(span, 2).item())
+                X *= (np.power(N, 1.0 / float(min(d, 3))) / 10.0) / radius
         else:
-            D, NN = spatial.cKDTree(X).query(X, k=k + 1, workers=-1)
+            X = Xin - Xin.mean(axis=0) if center else Xin.copy()
+            if rescale:
+                radius = 0.5 * np.linalg.norm(X.max(axis=0) - X.min(axis=0), 2)
+                X *= (np.power(N, 1.0 / float(min(d, 3))) / 10.0) / radius
+        if order is not None:
+            if on_device:
+                X = X[morton_order_device(X) if order == "morton"
+                      else torch.as_tensor(np.asarray(order), device=X.device).long()]
+            else:
+                X = X[morton_order(X) if order == "morton" else np.asarray(order)]
+        if backend is None:     # the device searches cover k <= 32
+            backend = "device" if k <= 32 else "host"
+        self.k = k
+        if backend == "device":
+            W, sigma = self._device_adjacency(X, k, sigma, p, epsilon, kwargs.get("dtype"),
+                                              kwargs.get("device"))
+        else:
+            W, sigma = self._host_adjacency(X.cpu().numpy() if on_device else X, k, sigma, p,
+                                            epsilon)
+        self.sigma = sigma
+        super().__init__(W, coords=X.cpu().numpy() if on_device else X, **kwargs)
+
+    def _device_adjacency(self, X, k, sigma, p, epsilon, dtype, device):
+        torch = nat.require_cuda()
+        dev, dt = _device_of(device), _torch_dtype(torch, dtype)
+        n = X.shape[0]
+        if self.NNtype == "knn":     # with 'average': the steps of knn_adjacency_device
+            nn, dist = knn_device(X, k, dev, p=p)
             if sigma is None:
-                sigma = np.mean(D[:, 1:])
-            self.k, self.sigma = k, sigma
-            rows = np.repeat(np.arange(N), k)
-            W = sparse.csr_matrix((np.exp(-D[:, 1:].ravel() ** 2 / float(sigma)),
-                                   (rows, NN[:, 1:].ravel())), shape=(N, N))
-            W = utils.symmetrize(W, "average").tocsr()
-        super().__init__(W, coords=X, **kwargs)
+                sigma = float(dist.mean().item())
+            indptr = torch.empty(n + 1, dtype=torch.int32, device=dev)
+            indices = torch.empty(n * k, dtype=torch.int32, device=dev)
+            data = torch.empty(n * k, dtype=dt, device=dev)
+            with torch.cuda.device(dev):
+                nat.call("gsp_knn_to_csr_" + nat.suffix(dt), nat.i64(n), nat.i32(k), nn, dist,
+                         nat.f64(sigma), indptr, indices, data, nat.stream_ptr(dev))
+            W = DeviceCSR(indptr, indices, data, (n, n))
+        else:
+            D = radius_device(X, epsilon, p, dev)
+            if sigma is None:
+                if D.nnz == 0:
+                    raise ValueError("No neighbors found")
+                sigma = float(D.data.mean().item())
+            W = _gauss_weights_device(D, sigma, dt)
+        return symmetrize_device(W, self.symmetrize_type), sigma
+
+    def _host_adjacency(self, X, k, sigma, p, epsilon):
+        N = X.shape[0]
+        if self.NNtype == "knn":
+            D, NN = _host_knn(X, k, p)
+            if sigma is None:
+                sigma = np.mean(D)
+            rows, cols, dist = np.repeat(np.arange(N), k), NN.ravel(), D.ravel()
+        else:
+            rows, cols, dist = _host_radius(X, epsilon, p)
+            if sigma is None:
+                if dist.size == 0:
+                    raise ValueError("No neighbors found")
+                sigma = np.mean(dist)
+        W = sparse.csr_matrix((np.exp(-dist ** 2 / float(sigma)), (rows, cols)), shape=(N, N))
+        return utils.symmetrize(W, self.symmetrize_type).tocsr(), sigma
+
+
+def _is_tensor(x):
+    return type(x).__module__.startswith("torch") and hasattr(x, "data_ptr")
+
+
+def _patch_pad_index(size, lo, hi):
+    """Source index of every position of np.pad(mode='symmetric') along one axis."""
+    i = np.arange(-lo, size + hi)
+    period = 2 * size
+    i = np.mod(i, period)
+    return np.where(i < size, i, period - 1 - i)
+
+
+def image_patches_device(img, patch_shape=(3, 3), device=None):
+    """Patch features of ImgPatches (imgpatches.py:51-105) as an (h*w, r*c*C) float64 CUDA
+    tensor: np.pad(img, mode='symmetric') with the reference's pad widths, then one row per
+    pixel in row-major order holding the r x c window (x C channels, channel fastest) --
+    skimage's view_as_windows + reshape, done by gather and unfold on the device."""
+    torch = nat.require_cuda()
+    dev = _device_of(device)
+    im = _device_points(img, dev) if not _is_tensor(img) else img.to(dev, torch.float64)
+    if im.dim() == 2:
+        im = im[:, :, None]
+    elif im.dim() != 3:
+        raise ValueError("Image should be a 2D (gray) or 3D (h, w, C) array.")
+    h, w, ch = im.shape
+    r, c = (patch_shape[0], patch_shape[1]) if len(patch_shape) > 1 else \
+        (patch_shape[0], patch_shape[0])
+    rows = _patch_pad_index(h, int((r - 0.5) / 2.0), int((r + 0.5) / 2.0))
+    cols = _patch_pad_index(w, int((c - 0.5) / 2.0), int((c + 0.5) / 2.0))
+    padded = im[torch.from_numpy(rows).to(dev)][:, torch.from_numpy(cols).to(dev)]
+    win = padded.unfold(0, r, 1).unfold(1, c, 1)          # (h, w, C, r, c)
+    return win.permute(0, 1, 3, 4, 2).reshape(h * w, r * c * ch).contiguous()
+
+
+class ImgPatches(NNGraph):
+    r"""Nearest-neighbour graph between the patches of an image (imgpatches.py:51-105).
+
+    Every pixel's feature vector is the ``patch_shape`` window centred on it (symmetric padding
+    at the borders), all channels stacked: ``r * c * C`` values for an (h, w, C) image, ``r * c``
+    for a gray one.  The features are built on the device (:func:`image_patches_device`) and
+    kept in ``Xin``; keyword arguments go to :class:`NNGraph`.
+    """
+
+    def __init__(self, img, patch_shape=(3, 3), **kwargs):
+        self.img = img
+        self.patch_shape = patch_shape
+        patches = image_patches_device(img, patch_shape, kwargs.get("device"))
+        super().__init__(patches, **kwargs)
+
+
+class Grid2dImgPatches(Graph):
+    r"""Union of a patch graph and the image's 2-D grid graph (grid2dimgpatches.py:37-43).
+
+    ``W = aggregate(Wp, Wg)`` of the :class:`ImgPatches` adjacency Wp and the
+    :class:`Grid2d` adjacency Wg.  The default ``Wp + Wg`` is summed on the device (COO
+    concatenation, then ``gsp_coo_to_csr_*``, which adds duplicates); a user-supplied
+    ``aggregate`` receives both as SciPy CSR matrices, as in the reference.  Keyword arguments
+    go to :class:`ImgPatches`; the graph takes the grid's coordinates.
+    """
+
+    def __init__(self, img, aggregate=None, **kwargs):
+        torch = nat.require_cuda()
+        h, w = img.shape[0], img.shape[1]
+        dt, dev = kwargs.get("dtype"), kwargs.get("device")
+        self.Gg = Grid2d(h, w, dtype=dt, device=dev)
+        self.Gp = ImgPatches(img, **kwargs)
+        if aggregate is None:
+            Wp, Wg = self.Gp.W, self.Gg.W
+            rows = torch.cat([_csr_rows(Wp), _csr_rows(Wg)])
+            cols = torch.cat([Wp.indices, Wg.indices])
+            vals = torch.cat([Wp.data, Wg.data.to(Wp.dtype)])
+            n = h * w
+            indptr = torch.empty(n + 1, dtype=torch.int32, device=Wp.device)
+            indices = torch.empty(vals.numel(), dtype=torch.int32, device=Wp.device)
+            data = torch.empty(vals.numel(), dtype=Wp.dtype, device=Wp.device)
+            uniq = ctypes.c_int64(0)
+            with torch.cuda.device(Wp.device):
+                nat.call("gsp_coo_to_csr_" + nat.suffix(Wp.dtype), nat.i64(n),
+                         nat.i64(vals.numel()), rows, cols, vals, indptr, indices, data,
+                         ctypes.byref(uniq), nat.stream_ptr(Wp.device))
+            m = int(uniq.value)
+            W = DeviceCSR(indptr, indices[:m].contiguous(), data[:m].contiguous(), (n, n))
+        else:
+            W = aggregate(self.Gp.W.to_scipy(), self.Gg.W.to_scipy())
+        super().__init__(W, coords=self.Gg.coords, plotting=self.Gg.plotting,
+                         dtype=dt, device=dev)
+
+
+def _csr_rows(M):
+    """Row id of every stored entry of a DeviceCSR (int32)."""
+    torch = nat.require_cuda()
+    counts = (M.indptr[1:] - M.indptr[:-1]).long()
+    return torch.repeat_interleave(torch.arange(M.shape[0], dtype=torch.int32,
+                                                device=M.device), counts)
 
 
 class Sensor(NNGraph):

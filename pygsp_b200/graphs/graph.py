@@ -464,6 +464,42 @@ def symmetrize_average_device(W):
     return DeviceCSR(sp, si, sd, W.shape)
 
 
+_SYMMETRIZE_MODES = {"maximum": 0, "fill": 1, "tril": 2, "triu": 3}
+
+
+def symmetrize_device(W, method="average"):
+    """utils.symmetrize(W, method) of a square DeviceCSR, on the device (utils.py:244-277).
+
+    'average' is :func:`symmetrize_average_device`; 'maximum', 'fill', 'tril' and 'triu' merge
+    each row of W with the same row of W^T (``gsp_csr_symmetrize_*``), with the reference's
+    arithmetic, so values are bit-equal to SciPy's in float64.  Exact zeros are dropped."""
+    if W.shape[0] != W.shape[1]:
+        raise ValueError("Matrix must be square.")
+    if method == "average":
+        return symmetrize_average_device(W)
+    if method not in _SYMMETRIZE_MODES:
+        raise ValueError("Unknown symmetrization method {}.".format(method))
+    torch = nat.require_cuda()
+    n, dev, sfx = W.shape[0], W.device, nat.suffix(W.dtype)
+    mode = nat.i32(_SYMMETRIZE_MODES[method])
+
+    def call(name, *args):
+        with torch.cuda.device(dev):
+            nat.call(name + "_" + sfx, *args, nat.stream_ptr(dev))
+    tp = torch.empty(n + 1, dtype=torch.int32, device=dev)
+    ti = torch.empty(W.nnz, dtype=torch.int32, device=dev)
+    td = torch.empty(W.nnz, dtype=W.dtype, device=dev)
+    call("gsp_csr_transpose", nat.i64(n), nat.i64(W.nnz), W.indptr, W.indices, W.data, tp, ti, td)
+    sp = torch.empty(n + 1, dtype=torch.int32, device=dev)
+    call("gsp_csr_symmetrize_count", nat.i64(n), mode, W.indptr, W.indices, W.data, tp, ti, td, sp)
+    nnz = int(sp[-1].item()) if n else 0
+    si = torch.empty(nnz, dtype=torch.int32, device=dev)
+    sd = torch.empty(nnz, dtype=W.dtype, device=dev)
+    call("gsp_csr_symmetrize_fill", nat.i64(n), mode, W.indptr, W.indices, W.data, tp, ti, td, sp,
+         si, sd)
+    return DeviceCSR(sp, si, sd, W.shape)
+
+
 def _torch_dtype(torch, dtype):
     if dtype is None:
         return torch.float32

@@ -52,8 +52,8 @@ def resistance_distance(G):
 def symmetrize(W, method="average"):
     """Host-side symmetrisation used by the graph generators (pygsp/utils.py:184-277).
 
-    Only the variants the generators on the path need: 'average' ((W+W^T)/2),
-    'maximum', 'tril' and 'triu' (mirror one triangle).
+    'average' ((W+W^T)/2), 'maximum', 'fill' (fill the zeros of each triangle from the
+    other, then average) and 'tril' / 'triu' (mirror one triangle).
     """
     if W.shape[0] != W.shape[1]:
         raise ValueError("Matrix must be square.")
@@ -63,6 +63,13 @@ def symmetrize(W, method="average"):
         if sparse.issparse(W):
             return W.maximum(W.T)
         return np.maximum(W, W.T)
+    if method == "fill":
+        A = W > 0
+        if sparse.issparse(W):
+            W = W + ((A + A.T) - A).multiply(W.T)
+        else:
+            W = W + np.logical_xor(np.logical_or(A, A.T), A) * W.T
+        return symmetrize(W, "average")
     if method in ("tril", "triu"):
         tri = getattr(sparse if sparse.issparse(W) else np, method)(W)
         return symmetrize(tri, "maximum")
