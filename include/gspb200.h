@@ -151,6 +151,42 @@ int gsp_cheby_step_halo_f32(int first, int64_t n_rows, int64_t nnz, const int32_
 GSPB200_DECLARE_CHEBY_API(f32, float)
 GSPB200_DECLARE_CHEBY_API(f64, double)
 
+/* Clenshaw filtering of ONE float32 source with the middle steps run two per launch.  A paired
+ * launch forms b_k into a third work block and b_{k-1} over b_{k+2} while b_k, b_{k+1} and the
+ * source are still in L2: five passes over a signal block per two steps instead of eight, and
+ * the same bits as gsp_cheby_clenshaw_f32, since every row is computed by the same instructions.
+ *
+ * gsp_cheby_pair_plan_host: the slot tables, once per (matrix, rows_per_tile).  Pure host code
+ *   on HOST copies of indptr / indices.  nbr_ptr (T + 1 entries, T = n / rows_per_tile) and
+ *   nbr_idx list per tile the tiles its rows reference and the tile itself; slots_fwd / slots_rev
+ *   (2 T entries each) are the launch orders of the two walk directions, (tile << 1) | step.  A
+ *   second-step tile is placed `lag` first-step tiles after the last one it reads, so that it
+ *   does not start while that one still runs on another CTA (the package passes 192: one
+ *   wave of 396 CTAs is 396 slots, about 198 first-step tiles).
+ *   *nbr_count_out receives the length of nbr_idx; when it exceeds nbr_capacity nothing else is
+ *   written and the caller calls again with that much room.  Each table is checked to place
+ *   every second-step tile after the first-step tiles it reads, else the call fails.
+ * gsp_cheby_clenshaw_pairs_wanted: 1 when pairing pays for an (n, nsig) float32 block under this
+ *   tile plan: the block exceeds the device's L2 (a block that fits is served from L2 by single
+ *   steps already).  GSPB200_CLENSHAW_PAIRS=0 / 1 forces the answer (A/B measurements, tests).
+ * gsp_cheby_clenshaw_pairs_f32: as gsp_cheby_clenshaw_f32 with nsrc = 1, but work holds
+ *   3*n*nsig elements, plan_host must hold a tiling, the four tables are DEVICE copies of the
+ *   plan, and tile_done is a device scratch array of T uint32 private to the call.  Every CTA of
+ *   a paired launch must be resident at once (the grid is sized so); a second-step tile polls
+ *   tile_done for a bounded time and traps if the first-step tiles it needs never finish. */
+int gsp_cheby_pair_plan_host(int64_t n, const int32_t* indptr_host, const int32_t* indices_host,
+                             int rows_per_tile, int lag, int64_t nbr_capacity, int32_t* nbr_ptr,
+                             int32_t* nbr_idx, int32_t* slots_fwd, int32_t* slots_rev,
+                             int64_t* nbr_count_out);
+int gsp_cheby_clenshaw_pairs_wanted(int64_t n, int64_t nsig, const gsp_tile_plan* plan_host);
+int gsp_cheby_clenshaw_pairs_f32(int64_t n, int64_t nnz, const int32_t* indptr,
+                                 const int32_t* indices, const float* data, double lmax,
+                                 const double* coeffs_host, int m, const float* source,
+                                 int64_t nsig, float* out, float* work,
+                                 const gsp_tile_plan* plan_host, const int32_t* slots_fwd,
+                                 const int32_t* slots_rev, const int32_t* nbr_ptr,
+                                 const int32_t* nbr_idx, uint32_t* tile_done, void* stream);
+
 /* ------------------------------------------------------------------- lmax ---
  * gsp_spmv_*: y = L x for ONE vector -- scipy's csr_matvec, the product ARPACK calls at
  *   pygsp/graphs/graph.py:911-917 and the one of graph.py:955.  2..32 lanes per row (from the

@@ -346,10 +346,26 @@ __global__ void combine_sources(int64_t count, const T* __restrict__ src, int ns
 // nsrc = 1 this is the single-filter Clenshaw evaluation (b_K = c_K x is folded into
 // the first step).  work holds 2*n*nsig elements.  Rounding differs from the forward
 // recurrence, the value does not (tests: same tolerance against the float64 oracle).
+//
+// With `pairs` (float32, one source, a tile plan; work then holds 3*n*nsig elements) the middle
+// steps k = K-3 .. 1 run two per launch (cheby_pair_tiled, csrc/cheby_tiled.cu): b_k goes to the
+// free third block, b_{k-1} over b_{k+2}, and the block of b_{k+1} becomes the free one.  The
+// first two steps, the last one and a left-over middle step are single launches.  Rows past the
+// last full tile take the row-group kernel: step A on them before the paired launch (it reads
+// only blocks complete by then, and the launch's B tiles gather its rows), step B after it.
+struct ClenshawPairs {
+  const int32_t* slots_fwd;
+  const int32_t* slots_rev;
+  const int32_t* nbr_ptr;
+  const int32_t* nbr_idx;
+  unsigned* tile_done;
+};
+
 template <typename T>
 int cheby_clenshaw(int64_t n, int64_t nnz, const int32_t* indptr, const int32_t* indices,
                    const T* vals, double lmax, const double* c, int nsrc, int m, const T* src,
-                   int nsig, T* out, T* work, const gsp_tile_plan* plan, cudaStream_t st) {
+                   int nsig, T* out, T* work, const gsp_tile_plan* plan, cudaStream_t st,
+                   const ClenshawPairs* pairs = nullptr) {
   GSP_REQUIRE(n >= 0 && nsig >= 1 && nsrc >= 1 && nsrc <= kMaxScales, "bad sizes");
   GSP_REQUIRE(m >= 2, "The coefficients have an invalid shape");
   GSP_REQUIRE(lmax > 0 && lmax == lmax, "lmax must be positive");
@@ -383,7 +399,40 @@ int cheby_clenshaw(int64_t n, int64_t nnz, const int32_t* indptr, const int32_t*
     k_next = K - 1;
   }
   s.r = const_cast<T*>(src);                      // read-only source blocks
+  T* spare = pairs ? work + 2 * n * int64_t(nsig) : nullptr;   // the third block of a paired call
+  unsigned launch_index = 0;
   for (int k = k_next; k >= 0; --k) {
+    if constexpr (std::is_same<T, float>::value) {
+      if (pairs && b_old && k >= 2) {
+        double ck2[kMaxScales];
+        Step<float> sa = s, sb = s;
+        clenshaw_coefs(sa, k, m, 1, lmax, c, ck);
+        clenshaw_coefs(sb, k - 1, m, 1, lmax, c, ck2);
+        sa.x_cur = b_cur; sa.x_old = b_old; sa.x_new = spare;
+        sb.x_cur = spare; sb.x_old = b_cur; sb.x_new = const_cast<float*>(b_old);
+        const int64_t tiles = n / plan->rows_per_tile;
+        if (launch_index == 0)
+          GSP_CUDA(cudaMemsetAsync(pairs->tile_done, 0, tiles * sizeof(unsigned), st));
+        const bool rev = (launch_index & 1) != 0;
+        PairLaunch pl{&sb, rev ? pairs->slots_rev : pairs->slots_fwd, pairs->nbr_ptr,
+                      pairs->nbr_idx, pairs->tile_done, ++launch_index};
+        const int64_t tiled_rows = tiles * plan->rows_per_tile;
+        int rc = cheby_step<float>(sa, tiled_rows, n, st);
+        if (rc != GSP_OK) return rc;
+        int64_t done = 0;
+        rc = cheby_step_tiled_f32(sa, 0, n, *plan, nullptr, &done, st, &pl);
+        if (rc != GSP_OK) return rc;
+        GSP_REQUIRE(done == tiled_rows, "the paired launch covers the full tiles");
+        rc = cheby_step<float>(sb, tiled_rows, n, st);
+        if (rc != GSP_OK) return rc;
+        float* freed = const_cast<float*>(b_cur);
+        b_cur = sb.x_new;
+        b_old = spare;
+        spare = freed;
+        --k;
+        continue;
+      }
+    }
     clenshaw_coefs(s, k, m, nsrc, lmax, c, ck);
     T* dst = k == 0 ? out : (b_old ? const_cast<T*>(b_old) : buf[1]);
     s.x_cur = b_cur;
@@ -487,6 +536,43 @@ extern "C" {
 
 GSP_CHEBY_API(f32, float)
 GSP_CHEBY_API(f64, double)
+
+int gsp_cheby_clenshaw_pairs_wanted(int64_t n, int64_t nsig, const gsp_tile_plan* plan_host) {
+  if (!plan_host || plan_host->rows_per_tile <= 0 || n / plan_host->rows_per_tile < 1) return 0;
+  const char* d = getenv("GSPB200_TILE_VDIR");           // probe: vectors staged by TMA, no pairs
+  if (d && *d && atoi(d) == 0) return 0;
+  const char* v = getenv("GSPB200_CLENSHAW_PAIRS");      // A/B probe: 0 never, 1 whatever the size
+  if (v && *v) return atoi(v) != 0;
+  int dev = 0, l2 = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess ||
+      cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, dev) != cudaSuccess)
+    return 0;
+  return n * nsig * int64_t(sizeof(float)) > int64_t(l2);
+}
+
+int gsp_cheby_clenshaw_pairs_f32(int64_t n, int64_t nnz, const int32_t* indptr,
+                                 const int32_t* indices, const float* data, double lmax,
+                                 const double* coeffs_host, int m, const float* source,
+                                 int64_t nsig, float* out, float* work,
+                                 const gsp_tile_plan* plan_host, const int32_t* slots_fwd,
+                                 const int32_t* slots_rev, const int32_t* nbr_ptr,
+                                 const int32_t* nbr_idx, uint32_t* tile_done, void* stream) {
+  GSP_REQUIRE(nsig >= 1 && nsig <= (1 << 20), "nsig out of range");
+  GSP_REQUIRE(plan_host && plan_host->rows_per_tile > 0, "paired steps need a tile plan");
+  GSP_REQUIRE(slots_fwd && slots_rev && nbr_ptr && nbr_idx && tile_done,
+              "paired steps need a pair plan");
+  gsp::Step<float> probe{nnz, indptr, indices, data};
+  probe.x_cur = work;
+  probe.x_old = work + n * nsig;
+  probe.x_new = work + 2 * n * nsig;
+  probe.r = const_cast<float*>(source);
+  probe.nscales = 1;
+  GSP_REQUIRE(gsp::tiled_step_applies(probe, 0, plan_host) && gsp::aligned16(out),
+              "paired steps need 16-byte aligned blocks");
+  const gsp::ClenshawPairs pairs{slots_fwd, slots_rev, nbr_ptr, nbr_idx, tile_done};
+  return gsp::cheby_clenshaw<float>(n, nnz, indptr, indices, data, lmax, coeffs_host, 1, m, source,
+                                    (int)nsig, out, work, plan_host, gsp::as_stream(stream), &pairs);
+}
 
 int gsp_cheby_step_halo_f32(int first, int64_t n_rows, int64_t nnz, const int32_t* indptr,
                             const int32_t* indices, const float* data, const float* x_cur,

@@ -64,6 +64,20 @@ struct TileArgs {
   int add_source;         // Clenshaw form: x_new += sum_i ck[i] * (tile i of r), r is not written
   const int64_t* out_perm;  // x_new row of local row i is out_perm[i] (NULL: i); last step of a partitioned call
   int vec_direct;           // x_old / r rows are read straight from global memory (not staged by TMA)
+  // Paired launch (cheby_pair_tiled): slot i runs tile slots[i] >> 1 as step A (bit 0 clear: the
+  // blocks above) or as step B (bit 0 set: the blocks below, which differ from A's in the three
+  // block pointers and in ck only).  B(t) starts once tile_done[s] >= done_target for every s in
+  // nbr_idx[nbr_ptr[t] .. nbr_ptr[t + 1]).
+  const int32_t* slots = nullptr;
+  int64_t n_slots = 0;
+  const int32_t* nbr_ptr = nullptr;
+  const int32_t* nbr_idx = nullptr;
+  unsigned* tile_done = nullptr;
+  unsigned done_target = 0;
+  const float* x_cur2 = nullptr;
+  const float* x_old2 = nullptr;
+  float* x_new2 = nullptr;
+  float ck2 = 0.f;
 };
 
 // ----------------------------------------------------------------- PTX helpers
@@ -162,10 +176,22 @@ __device__ __forceinline__ int64_t tile_of_slot(const TileArgs& a, int64_t slot)
 // partitioned step, a few per launch) gathers through L2 (ld.global.cg), never through the
 // non-coherent path.  Interior tiles only touch rows this GPU owns, which are read-only for the
 // whole launch: ld.global.nc.
-template <bool COH>
+// Step B of a paired launch gathers a block that step A writes during the same launch (each row
+// only after the acquire that proves it was written): a plain ld.global, cached in L1 like the
+// non-coherent gather but never turned into one by the compiler.
+__device__ __forceinline__ float4 ld_plain_f4(const float* p) {
+  float4 v;
+  asm volatile("ld.global.v4.f32 {%0, %1, %2, %3}, [%4];"
+               : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
+               : "l"(p));
+  return v;
+}
+constexpr int kGatherNc = 0, kGatherL2 = 1, kGatherPlain = 2;
+template <int COH>
 __device__ __forceinline__ float4 gather_f4(const float* __restrict__ xg, int col, int ns) {
   const float* p = xg + int64_t(col) * ns;
-  if (COH) return __ldcg(reinterpret_cast<const float4*>(p));
+  if (COH == kGatherL2) return __ldcg(reinterpret_cast<const float4*>(p));
+  if (COH == kGatherPlain) return ld_plain_f4(p);
   return ldg_f4(p);
 }
 
@@ -180,7 +206,7 @@ __device__ __forceinline__ float4 gather_f4(const float* __restrict__ xg, int co
 // are in flight per lane at a time (the same 64 bytes either way).
 // COH: the row may reference halo columns (boundary tiles of a partitioned step) -- the tile
 // gathers through L2 then; interior tiles use the plain non-coherent gather only.
-template <int G, int P, bool COH>
+template <int G, int P, int COH>
 __device__ __forceinline__ void row_gather_sum(const int32_t* __restrict__ sm_col,
                                                const float* __restrict__ sm_val, int jb, int je,
                                                const float* __restrict__ xg, float4 (&acc)[P]) {
@@ -244,24 +270,32 @@ __device__ __forceinline__ void fma4(float4& d, float w, const float4& v) {
 
 // The rows of one tile: gather + three-term recurrence + coefficient AXPYs + stores.
 // COH: the tile's rows may reference halo columns (coherent gathers through L2).
-template <int G, bool FIRST, int NSC, bool COH, int P>
+// PAIR (paired launch): 1 = step A, 2 = step B.  B takes its blocks and ck from the second operand
+// set and reads the gathered block, which A writes in the same launch, with plain loads.  A reads
+// the source rows through L2 without the evict-first mark, since B reads them again.
+template <int G, bool FIRST, int NSC, int COH, int P, int PAIR = 0>
 __device__ __forceinline__ void tile_rows(const TileArgs& a, const TileCtx t) {
+  const float* x_cur_blk = PAIR == 2 ? a.x_cur2 : a.x_cur;
+  const float* x_old_blk = PAIR == 2 ? a.x_old2 : a.x_old;
+  float* x_new_blk = PAIR == 2 ? a.x_new2 : a.x_new;
   constexpr int RP = 32 / G;               // rows in flight per warp
   constexpr int NS = 4 * G * P;            // signal columns (compile-time: cheap addressing)
   constexpr int PS = 4 * G;                // column distance between a lane's packets
   const int R = a.rows_per_tile;
   const int NW = a.consumer_warps;
   const int c0 = t.c0;
-  const float* __restrict__ xg = a.x_cur + c0;      // this lane's first column packet of x_cur
+  const float* __restrict__ xg = x_cur_blk + c0;    // this lane's first column packet of x_cur
   const int nscales = NSC >= 0 ? NSC : a.nscales;
   const float alpha = a.alpha, beta = a.beta, gamma = a.gamma;
-  const bool keep_writes = a.keep_writes != 0;
+  // (B's stores are evict-first: nothing reads them before the next launch, and L2 is what the
+  //  pair lives on; config 2, H100: 12.25 -> 12.02 ms per call)
+  const bool keep_writes = a.keep_writes != 0 && PAIR != 2;
   const bool VD = t.vd;
   const float* sm_vec = t.sm_vec;
   const int a0 = t.sm_ptr[R + 4];
   const int64_t r0 = t.r0;
   const float* __restrict__ xc_tile = xg + r0 * NS;
-  float* __restrict__ xn_tile = a.x_new + r0 * NS + c0;
+  float* __restrict__ xn_tile = x_new_blk + r0 * NS + c0;
   float* __restrict__ r_tile = a.r + r0 * NS + c0;
   const int64_t r_stride = a.r_rows * NS;
 
@@ -271,7 +305,8 @@ __device__ __forceinline__ void tile_rows(const TileArgs& a, const TileCtx t) {
     const int je = t.sm_ptr[lr + 1] - a0;
     float4 xc[P];
 #pragma unroll
-    for (int p = 0; p < P; ++p) xc[p] = ldg_f4(xc_tile + off + p * PS);
+    for (int p = 0; p < P; ++p)
+      xc[p] = COH == kGatherPlain ? ld_plain_f4(xc_tile + off + p * PS) : ldg_f4(xc_tile + off + p * PS);
     // direct mode: this row's x_old and first r / source packets are requested now (streaming
     // loads, no L1 allocation) and consumed after the gather loop, which hides their latency
     float4 xo_d[P], r0_d[P];
@@ -280,9 +315,11 @@ __device__ __forceinline__ void tile_rows(const TileArgs& a, const TileCtx t) {
     if (!FIRST && VD) {
 #pragma unroll
       for (int p = 0; p < P; ++p) {
-        xo_d[p] = __ldcs(reinterpret_cast<const float4*>(a.x_old + (r0 + lr) * NS + c0 + p * PS));
-        if (NSC != 0 && nscales > 0)
-          r0_d[p] = __ldcs(reinterpret_cast<const float4*>(a.r + (r0 + lr) * NS + c0 + p * PS));
+        xo_d[p] = __ldcs(reinterpret_cast<const float4*>(x_old_blk + (r0 + lr) * NS + c0 + p * PS));
+        if (NSC != 0 && nscales > 0) {
+          const float4* rp = reinterpret_cast<const float4*>(a.r + (r0 + lr) * NS + c0 + p * PS);
+          r0_d[p] = PAIR == 1 ? __ldcg(rp) : __ldcs(rp);
+        }
       }
     }
     float4 acc[P];
@@ -305,7 +342,7 @@ __device__ __forceinline__ void tile_rows(const TileArgs& a, const TileCtx t) {
 #pragma unroll
       for (int i = 0; i < (NSC >= 0 ? NSC : kTiledMaxScales); ++i) {
         if (NSC < 0 && i >= nscales) break;
-        const float w = a.ck[i];
+        const float w = PAIR == 2 ? a.ck2 : a.ck[i];
 #pragma unroll
         for (int p = 0; p < P; ++p) {
           const float4 sv =
@@ -318,7 +355,7 @@ __device__ __forceinline__ void tile_rows(const TileArgs& a, const TileCtx t) {
       }
     }
     if (a.out_perm) {    // the caller's row order: local row -> original row (uniform branch)
-      float* dst = a.x_new + __ldg(a.out_perm + r0 + lr) * NS + c0;
+      float* dst = x_new_blk + __ldg(a.out_perm + r0 + lr) * NS + c0;
 #pragma unroll
       for (int p = 0; p < P; ++p) store_f4(dst + p * PS, xn[p], keep_writes);
     } else {
@@ -383,7 +420,7 @@ __device__ __noinline__ void boundary_tile(const TileArgs& a, const TileCtx t, i
     }
     __syncwarp();
   }
-  tile_rows<G, FIRST, NSC, true, 1>(a, t);
+  tile_rows<G, FIRST, NSC, kGatherL2, 1>(a, t);
   if (t.tile >= a.halo.n_push_tiles) return;
   if (!a.out_perm) {
     const float* xn_tile = a.x_new + t.r0 * NS + t.c0;
@@ -547,9 +584,143 @@ cheby_step_tiled(const __grid_constant__ TileArgs a) {
     if (HALO && tile < a.n_front)          // warp-uniform; interior tiles never wait
       boundary_tile<G, FIRST, NSC>(a, t, lane);
     else
-      tile_rows<G, FIRST, NSC, false, P>(a, t);
+      tile_rows<G, FIRST, NSC, kGatherNc, P>(a, t);
     __syncwarp();
     if (lane == 0) mbar_arrive(empty + s);
+  }
+}
+
+// Two middle Clenshaw steps in one launch (float32, one source, direct vectors, one-stage ring).
+// Step A forms b_k = a2 L P - 2 P - Q + c_k x into a third block W; step B forms
+// b_{k-1} = a2 L W - 2 W - P + c_{k-1} x over Q.  The CTAs walk a slot table (built once per
+// matrix, csrc/pair_plan.cu) round-robin: the A tiles in walk order, and B(t) a fixed lag after
+// the last A tile among t and the tiles t's rows reference -- late enough that those A tiles are
+// done when B(t) starts (slots that are neighbours in the table run at the same time on
+// different CTAs), early enough that W, P and x are still in L2: five passes over a signal block
+// per pair instead of eight.  No block is both gathered and written in the launch: P and x are
+// read-only, W is written by A and read by B only, and the rows of Q that B(t) overwrites are
+// read by A(t) alone.  Per row the instructions are those of the single step: the same bits.
+//
+// An acquire at GPU scope makes the SM drop its L1 (CCTL.IVALL), which the gathers of all resident
+// CTAs live on, so it is paid once per B tile and CTA and never inside a poll loop: consumer warp
+// 0 polls with relaxed loads, fences once, and a named barrier hands the tile to the other
+// consumer warps.  On the release side each warp's stores are ordered by __syncwarp before lane
+// 0's red.release (a fence without L1 invalidation).
+template <int G, int P>
+__global__ void __launch_bounds__(32 * (P == 2 ? 9 : 17), P == 2 ? 3 : 2)
+cheby_pair_tiled(const __grid_constant__ TileArgs a) {
+  extern __shared__ __align__(128) unsigned char smem[];
+  const int R = a.rows_per_tile;
+  const int NW = a.consumer_warps;
+  const TileLayout lay(R, a.slab_cap, a.nsig, a.nscales, true, 1);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem);
+  uint64_t* empty = full + 1;
+  unsigned char* st = smem + lay.bar_bytes;
+  int32_t* sm_col = reinterpret_cast<int32_t*>(st);
+  float* sm_val = reinterpret_cast<float*>(st + lay.slab_bytes);
+  int32_t* sm_ptr = reinterpret_cast<int32_t*>(st + 2 * lay.slab_bytes);
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) {
+    mbar_init(full, 1);
+    mbar_init(empty, NW);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  if (warp == 0) {
+    // producer: the CSR slab of the slot's tile (the same slab for A(t) and B(t)); the slot table
+    // and the tile's first / last CSR offsets are read one slot ahead
+    if (lane != 0) return;
+    const bool hint = a.l2_hint != 0;
+    const uint64_t pol = l2_policy_evict_first();
+    int64_t ntile = 0;
+    int nbegin = 0, nend = 0, ncode = 0;
+    if (int64_t(blockIdx.x) < a.n_slots) {
+      ncode = __ldg(a.slots + blockIdx.x);
+      ntile = ncode >> 1;
+      nbegin = __ldg(a.indptr + a.row_begin + ntile * R);
+      nend = __ldg(a.indptr + a.row_begin + ntile * R + R);
+    }
+    uint32_t it = 0;
+    for (int64_t slot = blockIdx.x; slot < a.n_slots; slot += gridDim.x, ++it) {
+      const int64_t tile = ntile;
+      const int begin = nbegin, end = nend;
+      const bool evict = hint && (ncode & 1);     // A's slab stays in L2 for B(t): 12.16 -> 12.02 ms
+      if (slot + gridDim.x < a.n_slots) {
+        ncode = __ldg(a.slots + slot + gridDim.x);
+        ntile = ncode >> 1;
+        nbegin = __ldg(a.indptr + a.row_begin + ntile * R);
+        nend = __ldg(a.indptr + a.row_begin + ntile * R + R);
+      }
+      mbar_wait(empty, (it & 1u) ^ 1u);
+      const int64_t r0 = a.row_begin + tile * R;
+      const int a0 = begin & ~3;
+      int a1 = (end + 3) & ~3;
+      if (int64_t(a1) > a.nnz) a1 = end & ~3;
+      sm_ptr[R] = end;
+      sm_ptr[R + 4] = a0;
+      for (int k = (a1 > a0 ? a1 : a0); k < end; ++k) {
+        sm_col[k - a0] = __ldg(a.indices + k);
+        sm_val[k - a0] = __ldg(a.vals + k);
+      }
+      const uint32_t slab = a1 > a0 ? uint32_t(a1 - a0) * 4u : 0u;
+      mbar_expect_tx(full, uint32_t(R) * 4u + 2u * slab);
+      bulk_g2s(sm_ptr, a.indptr + r0, uint32_t(R) * 4u, full);
+      if (slab && evict) {
+        bulk_g2s_hint(sm_col, a.indices + a0, slab, full, pol);
+        bulk_g2s_hint(sm_val, a.vals + a0, slab, full, pol);
+      } else if (slab) {
+        bulk_g2s(sm_col, a.indices + a0, slab, full);
+        bulk_g2s(sm_val, a.vals + a0, slab, full);
+      }
+    }
+    return;
+  }
+
+  const int cw = warp - 1;
+  const int sub = lane / G;
+  const int c0 = (lane % G) * 4;
+  uint32_t it = 0;
+  for (int64_t slot = blockIdx.x; slot < a.n_slots; slot += gridDim.x, ++it) {
+    const int code = __ldg(a.slots + slot);
+    const int64_t tile = code >> 1;
+    mbar_wait(full, it & 1u);
+    const TileCtx t = {nullptr, sm_col, sm_val, sm_ptr, tile, a.row_begin + tile * R, cw, sub, c0, true};
+    if (code & 1) {
+      // Wait until every A tile that B(tile) reads is stored.  This cannot deadlock: all CTAs of
+      // the grid are resident (the launch requires it), each walks its slots in increasing order,
+      // a B slot waits only for A tiles in lower slots (checked when the table is built), and an
+      // A slot waits for nothing; so the lowest unfinished slot of the launch can always finish.
+      // The poll is bounded all the same: a wait of seconds can only be a broken table, and a
+      // trapped launch is reported to the caller where a spinning one would hold the device.
+      if (cw == 0) {
+        const int e1 = __ldg(a.nbr_ptr + tile + 1);
+        for (int e = __ldg(a.nbr_ptr + tile) + lane; e < e1; e += 32) {
+          const unsigned* f = a.tile_done + __ldg(a.nbr_idx + e);
+          unsigned seen, polls = 0;
+          for (;;) {
+            asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(seen) : "l"(f) : "memory");
+            if (seen >= a.done_target) break;
+            if (++polls > (1u << 24)) __trap();
+            __nanosleep(128);
+          }
+        }
+        __syncwarp();
+        asm volatile("fence.acq_rel.gpu;" ::: "memory");
+      }
+      asm volatile("bar.sync 1, %0;" ::"r"(NW * 32) : "memory");
+      tile_rows<G, false, 1, kGatherPlain, P, 2>(a, t);
+    } else {
+      tile_rows<G, false, 1, kGatherNc, P, 1>(a, t);
+      // publish: the warp's stores, then its arrival (the tile is done at NW arrivals)
+      __syncwarp();
+      if (lane == 0)
+        asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(a.tile_done + tile) : "memory");
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(empty);
   }
 }
 
@@ -659,8 +830,35 @@ static int launch_tiled_g(bool first, const TileArgs& a, bool halo, bool two, in
   return launch_tiled_gh<G, false, 1>(first, a, bps, st);
 }
 
+template <int G, int P>
+static int launch_pair_k(const TileArgs& a, int blocks_per_sm, cudaStream_t st) {
+  const TileLayout lay(a.rows_per_tile, a.slab_cap, a.nsig, a.nscales, true, 1);
+  const int smem = lay.total(1);
+  const int threads = 32 * (1 + a.consumer_warps);
+  GSP_REQUIRE(threads <= 32 * (P == 2 ? 9 : 17), "too many consumer warps for this mapping");
+  auto kern = cheby_pair_tiled<G, P>;
+  GSP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  int per_sm = 0;
+  GSP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem));
+  // B tiles wait for A tiles of other CTAs: every CTA of the grid must be resident
+  GSP_REQUIRE(per_sm >= 1, "paired tiled kernel does not fit");
+  if (blocks_per_sm > 0) per_sm = std::min(per_sm, blocks_per_sm);
+  const int64_t grid = std::min<int64_t>(a.n_slots, int64_t(sm_count()) * per_sm);
+  kern<<<(unsigned)grid, threads, smem, st>>>(a);
+  GSP_LAUNCH_CHECK("cheby_pair_tiled");
+  return GSP_OK;
+}
+
+// the lane mappings of launch_tiled_g without a halo
+template <int G>
+static int launch_pair_g(const TileArgs& a, bool two, int bps, cudaStream_t st) {
+  if (two && G >= 8) return launch_pair_k<(G >= 8 ? G / 2 : G), (G >= 8 ? 2 : 1)>(a, bps, st);
+  return launch_pair_k<G, 1>(a, bps, st);
+}
+
 int cheby_step_tiled_f32(const Step<float>& s, int64_t rb, int64_t re, const gsp_tile_plan& plan,
-                         const gsp_halo_fusion* halo, int64_t* rows_done, cudaStream_t st) {
+                         const gsp_halo_fusion* halo, int64_t* rows_done, cudaStream_t st,
+                         const PairLaunch* pair) {
   const bool first = s.first;
   const int nsig = s.nsig, nscales = s.nscales;
   TileArgs a;
@@ -675,7 +873,7 @@ int cheby_step_tiled_f32(const Step<float>& s, int64_t rb, int64_t re, const gsp
   memset(&a.halo, 0, sizeof(a.halo));
   const int64_t full_tiles = (re - rb) / plan.rows_per_tile;
   gsp_halo_fusion probe;                       // GSPB200_FORCE_HALO=1: run the halo-capable
-  if (!halo && rb == 0 && env_int("GSPB200_FORCE_HALO", 0)) {   // variant with no neighbours
+  if (!halo && !pair && rb == 0 && env_int("GSPB200_FORCE_HALO", 0)) {   // variant with no neighbours
     memset(&probe, 0, sizeof(probe));          // (single-GPU A/B of the two instantiations)
     probe.n_owned = 0x7fffffff;
     halo = &probe;
@@ -728,6 +926,29 @@ int cheby_step_tiled_f32(const Step<float>& s, int64_t rb, int64_t re, const gsp
   // bank at order 50 on a grid 89.8 / 97.1 -> 84.0 / 84.1 ms.  So two packets are the default.
   const bool two = !h && nsig >= 32 && env_int("GSPB200_TILE_P2", 1) != 0;
   if (two) a.consumer_warps = std::min(a.consumer_warps, 8);
+  if (pair) {
+    const Step<float>& b = *pair->second;
+    GSP_REQUIRE(!h && !first && s.add_source && nscales == 1 && a.vec_direct && !s.out_perm,
+                "a paired launch takes two middle Clenshaw steps of one source");
+    GSP_REQUIRE(float(b.alpha) == a.alpha && float(b.beta) == a.beta && float(b.gamma) == a.gamma,
+                "paired steps share alpha, beta and gamma");
+    GSP_REQUIRE(a.n_tiles < (int64_t(1) << 30), "too many tiles for the slot table");
+    a.slots = pair->slots;
+    a.n_slots = 2 * a.n_tiles;
+    a.nbr_ptr = pair->nbr_ptr;
+    a.nbr_idx = pair->nbr_idx;
+    a.tile_done = pair->tile_done;
+    a.done_target = pair->launch_index * unsigned(a.consumer_warps);
+    a.x_cur2 = b.x_cur; a.x_old2 = b.x_old; a.x_new2 = b.x_new;
+    a.ck2 = float(b.ck[0]);
+    switch (nsig) {
+      case 8: return launch_pair_g<2>(a, false, plan.blocks_per_sm, st);
+      case 16: return launch_pair_g<4>(a, false, plan.blocks_per_sm, st);
+      case 32: return launch_pair_g<8>(a, two, plan.blocks_per_sm, st);
+      case 64: return launch_pair_g<16>(a, two, plan.blocks_per_sm, st);
+      case 128: return launch_pair_g<32>(a, two, plan.blocks_per_sm, st);
+    }
+  }
   switch (nsig) {
     case 8: return launch_tiled_g<2>(first, a, h, false, plan.blocks_per_sm, st);
     case 16: return launch_tiled_g<4>(first, a, h, false, plan.blocks_per_sm, st);

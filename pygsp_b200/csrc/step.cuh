@@ -73,8 +73,20 @@ int cheby_step(const Step<T>& s, int64_t rb, int64_t re, cudaStream_t st);
 // The tiled kernel on the full tiles of [rb, re) (rb % 4 == 0); reports the rows done.  With a halo
 // (rb == 0) it runs the halo-capable instantiation, whose first tiles wait, push and publish as
 // gsp_halo_fusion says.
+// With `pair`, one launch runs step s (A) and step *pair->second (B, the step that follows A) on
+// the full tiles: see cheby_pair_tiled.  The two are middle Clenshaw steps of one source; B gathers
+// the block A writes, which is neither of A's input blocks.
+struct PairLaunch {
+  const Step<float>* second;
+  const int32_t* slots;      // 2 * tiles entries of gsp_cheby_pair_plan_host, in the walk direction
+  const int32_t* nbr_ptr;
+  const int32_t* nbr_idx;
+  unsigned* tile_done;       // one counter per tile, zero before launch_index 1
+  unsigned launch_index;     // 1, 2, ... over the launches that share tile_done
+};
 int cheby_step_tiled_f32(const Step<float>& s, int64_t rb, int64_t re, const gsp_tile_plan& plan,
-                         const gsp_halo_fusion* halo, int64_t* rows_done, cudaStream_t st);
+                         const gsp_halo_fusion* halo, int64_t* rows_done, cudaStream_t st,
+                         const PairLaunch* pair = nullptr);
 
 // Forward recurrence (approximations.py:99-112), step k = 1 .. m-1 of coefficient rows c
 // (nscales x m): T_k = (4/lmax) L T_{k-1} - 2 T_{k-1} - T_{k-2} and r_i += c_ik T_k; the first step

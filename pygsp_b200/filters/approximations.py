@@ -6,6 +6,8 @@ and ``cheby_rect`` (:117-163).  The recurrence runs in ``libgspb200``:
 one fused CUDA kernel per order (csrc/cheby.cu) instead of SciPy's
 ``csr_matvecs`` + NumPy temporaries + fancy-indexed accumulation.
 """
+import ctypes
+
 import numpy as np
 
 from .. import _native as nat
@@ -121,7 +123,8 @@ def cheby_clenshaw_device(L, lmax, c, sources, out=None, work=None):
     nsrc = Nf sources it is the *synthesis* of ``Filter.filter`` in K SpMMs instead of the
     reference's Nf * K (filter.py:313-322), because Clenshaw's recurrence is linear in its
     source term: b_k = sum_i c_ik s_i + 2 Lt b_{k+1} - b_{k+2}  (SURVEY.md 8f).
-    Returns (N, nsig).
+    Returns (N, nsig).  ``work`` is (2, N, nsig); with (3, N, nsig), or none, a single float32
+    source on a block larger than L2 runs its middle steps two per launch (same bits).
     """
     torch = nat.require_cuda()
     c = np.ascontiguousarray(np.atleast_2d(np.asarray(c, dtype=np.float64)))
@@ -137,9 +140,23 @@ def cheby_clenshaw_device(L, lmax, c, sources, out=None, work=None):
     sources = sources.contiguous()
     if out is None:
         out = torch.empty((n, nsig), dtype=L.dtype, device=L.device)
+    plan = L.tile_plan(nsig, nsrc)
+    # one float32 source on a block larger than L2: the middle steps run two per launch, which
+    # takes a third work block (a caller's two-block work keeps the single steps)
+    if (nsrc == 1 and plan is not None and (work is None or work.shape[0] >= 3)
+            and nat.lib().gsp_cheby_clenshaw_pairs_wanted(nat.i64(n), nat.i64(nsig),
+                                                          ctypes.byref(plan))):
+        if work is None:
+            work = torch.empty((3, n, nsig), dtype=L.dtype, device=L.device)
+        tables = L.pair_plan(plan.rows_per_tile)
+        tile_done = torch.empty(n // plan.rows_per_tile, dtype=torch.int32, device=L.device)
+        with torch.cuda.device(L.device):
+            nat.call("gsp_cheby_clenshaw_pairs_f32", nat.i64(n), nat.i64(L.nnz), L.indptr,
+                     L.indices, L.data, nat.f64(lmax), c, nat.i32(c.shape[1]), sources,
+                     nat.i64(nsig), out, work, plan, *tables, tile_done, nat.stream_ptr(L.device))
+        return out
     if work is None:
         work = torch.empty((2, n, nsig), dtype=L.dtype, device=L.device)
-    plan = L.tile_plan(nsig, nsrc)
     with torch.cuda.device(L.device):
         nat.call("gsp_cheby_clenshaw_" + nat.suffix(L.dtype), nat.i64(n), nat.i64(L.nnz),
                  L.indptr, L.indices, L.data, nat.f64(lmax), c, nat.i32(nsrc),

@@ -34,6 +34,36 @@ class DeviceCSR:
             self._plans[key] = plan if plan.rows_per_tile > 0 else None
         return self._plans[key]
 
+    def pair_plan(self, rows_per_tile):
+        """Slot tables of the paired Clenshaw launch for this matrix (cached): the device tensors
+        (slots_fwd, slots_rev, nbr_ptr, nbr_idx) of ``gsp_cheby_pair_plan_host``, which runs on a
+        host copy of the structure.  GSPB200_PAIR_LAG overrides the lag (a probe)."""
+        import ctypes
+        import os
+        torch = nat.require_cuda()
+        lag = int(os.environ.get("GSPB200_PAIR_LAG") or 192)
+        key = ("pairs", int(rows_per_tile), lag)
+        if key not in self._plans:
+            indptr = self.indptr.cpu().numpy()
+            indices = self.indices.cpu().numpy()
+            n, T = self.shape[0], self.shape[0] // int(rows_per_tile)
+            count = ctypes.c_int64(0)
+            cap = 16 * T
+            while True:
+                nbr_ptr = np.empty(T + 1, dtype=np.int32)
+                nbr_idx = np.empty(cap, dtype=np.int32)
+                fwd = np.empty(2 * T, dtype=np.int32)
+                rev = np.empty(2 * T, dtype=np.int32)
+                nat.call("gsp_cheby_pair_plan_host", nat.i64(n), indptr, indices,
+                         nat.i32(rows_per_tile), nat.i32(lag), nat.i64(cap), nbr_ptr, nbr_idx,
+                         fwd, rev, ctypes.byref(count))
+                if count.value <= cap:
+                    break
+                cap = count.value
+            self._plans[key] = tuple(torch.from_numpy(a).to(self.device)
+                                     for a in (fwd, rev, nbr_ptr, nbr_idx[:max(count.value, 1)]))
+        return self._plans[key]
+
     # -- construction ---------------------------------------------------------
     @classmethod
     def from_scipy(cls, M, dtype, device):
