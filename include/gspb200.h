@@ -486,8 +486,9 @@ int gsp_cheby_op_dist_f64(const gsp_dist_plan* plan_host, const gsp_tile_plan* t
  * gsp_knn_grid: k nearest neighbours (self excluded) of n points in 2-D / 3-D by a
  *     uniform cell grid -- the scipy.spatial.KDTree query of nngraph.py:213-216 for the
  *     Euclidean metric; other dimensions and metrics: gsp_knn_brute below.
- *     points (n, dim) double; lo/hi: bounding box, cells: grid resolution (host arrays
- *     of length dim); outputs (n, k) row-major, ascending distance, ties by index.
+ *     points (n, dim) double; lo/hi: bounding box (finite), cells: grid resolution, 1 .. 2^30
+ *     per axis and < 2^31 in all (host arrays of length dim); outputs (n, k) row-major,
+ *     ascending distance, ties by index: the lists of gsp_knn_brute(p = 2), bit for bit.
  * gsp_knn_to_csr_*: directed k-NN matrix W[i, nn] = exp(-d^2/sigma) as CSR with sorted
  *     rows (nngraph.py:221-226,289); symmetrise with gsp_csr_transpose / _average.
  */

@@ -54,10 +54,15 @@ __global__ void grid2d_fill_kernel(int64_t n1, int64_t n2, const int32_t* __rest
 }
 
 // ------------------------------------------------------------------------ kNN
+// Cells per axis are bounded by kMaxAxisCells, so home +- ring (ring <= the largest axis) stays
+// in int32.
+constexpr int kMaxAxisCells = 1 << 30;
+
 struct GridSpec {
   double lo[3];
   double inv_h[3];
   double h[3];
+  double slack[3];   // 2^-44 max(|lo|, |hi|): rounding margin of the stopping test
   int cells[3];
   int dim;
 };
@@ -122,25 +127,26 @@ __global__ void knn_query_kernel(int64_t n, int k, GridSpec g,
   int max_ring = max(g.cells[0], g.cells[1]);
   if (zdim) max_ring = max(max_ring, g.cells[2]);
   for (int ring = 0; ring <= max_ring; ++ring) {
+    // the cells at Chebyshev distance `ring` from home, clipped to the grid
+    const int x0 = home[0] - ring, x1 = home[0] + ring, y0 = home[1] - ring, y1 = home[1] + ring;
     const int z0 = zdim ? home[2] - ring : 0, z1 = zdim ? home[2] + ring : 0;
-    for (int cz = z0; cz <= z1; ++cz) {
-      if (zdim && (cz < 0 || cz >= g.cells[2])) continue;
-      for (int cy = home[1] - ring; cy <= home[1] + ring; ++cy) {
-        if (cy < 0 || cy >= g.cells[1]) continue;
-        const bool edge_zy = (zdim && (cz == z0 || cz == z1)) || cy == home[1] - ring ||
-                             cy == home[1] + ring;
-        // on an inner (z, y) line only the two end cells belong to this ring
-        const int step = edge_zy ? 1 : max(2 * ring, 1);
-        for (int cx = home[0] - ring; cx <= home[0] + ring; cx += step) {
-          if (cx < 0 || cx >= g.cells[0]) continue;
+    for (int cz = max(z0, 0); cz <= min(z1, g.cells[2] - 1); ++cz) {
+      for (int cy = max(y0, 0); cy <= min(y1, g.cells[1] - 1); ++cy) {
+        // on a face of the ring's box every cell belongs to the ring, on an inner (z, y) line
+        // only the two end cells x0 and x1
+        const bool face = (zdim && (cz == z0 || cz == z1)) || cy == y0 || cy == y1;
+        for (int cx = face ? max(x0, 0) : x0; cx <= min(x1, g.cells[0] - 1);
+             cx = (face || cx == x1) ? cx + 1 : x1) {
+          if (cx < 0) continue;
           const int64_t cell = (int64_t(cz) * g.cells[1] + cy) * g.cells[0] + cx;
           for (int q = cell_start[cell]; q < cell_start[cell + 1]; ++q) {
             const int cand = sorted_ids[q];
             if (cand == self) continue;
+            // squares summed in dimension order by FMA: gsp_knn_brute's arithmetic, bit for bit
             double d2 = 0;
             for (int d = 0; d < g.dim; ++d) {
               const double diff = sp[int64_t(q) * g.dim + d] - p[d];
-              d2 += diff * diff;
+              d2 = fma(diff, diff, d2);
             }
             if (found == k && !(d2 < best_d[k - 1] || (d2 == best_d[k - 1] && cand < best_i[k - 1])))
               continue;
@@ -159,15 +165,26 @@ __global__ void knn_query_kernel(int64_t n, int k, GridSpec g,
       }
     }
     if (found == k) {
-      // every unvisited point lies outside the box of cells searched so far
-      double reach = 1e300;
+      // Every unvisited point lies in a cell outside the box searched so far, so it is at least
+      // `reach` away, less rounding: a point binned at or above cell c has
+      // fl(fl(x - lo) * fl(1 / h)) >= c, so x >= lo + c h (1 - 3u) (and symmetrically below), and
+      // the face lo + c h and the distance to it are rounded once each.  Both errors are below 2^-48 max(|lo|, |hi|), and
+      // slack = 2^-44 max(|lo|, |hi|) leaves room for the rounding of d^2 too: the d^2 of every
+      // unvisited point is strictly above reach^2, so a tie at the k-th distance is always seen.
+      double reach = INFINITY;
       bool whole = true;
       for (int d = 0; d < g.dim; ++d) {
         const int lo_c = home[d] - ring, hi_c = home[d] + ring;
-        if (lo_c > 0) { reach = fmin(reach, p[d] - (g.lo[d] + lo_c * g.h[d])); whole = false; }
-        if (hi_c < g.cells[d] - 1) { reach = fmin(reach, (g.lo[d] + (hi_c + 1) * g.h[d]) - p[d]); whole = false; }
+        if (lo_c > 0) {
+          reach = fmin(reach, p[d] - fma(double(lo_c), g.h[d], g.lo[d]) - g.slack[d]);
+          whole = false;
+        }
+        if (hi_c < g.cells[d] - 1) {
+          reach = fmin(reach, fma(double(hi_c + 1), g.h[d], g.lo[d]) - p[d] - g.slack[d]);
+          whole = false;
+        }
       }
-      if (whole || best_d[k - 1] <= reach * reach) break;
+      if (whole || (reach > 0 && best_d[k - 1] < reach * reach)) break;
     }
   }
   for (int j = 0; j < k; ++j) {
@@ -244,12 +261,15 @@ int gsp_knn_grid(int64_t n, int dim, const double* points, int k, const double* 
   int64_t ncells = 1;
   for (int d = 0; d < 3; ++d) {
     g.cells[d] = d < dim ? cells_host[d] : 1;
-    GSP_REQUIRE(g.cells[d] >= 1, "cells must be positive");
+    GSP_REQUIRE(g.cells[d] >= 1 && g.cells[d] <= gsp::kMaxAxisCells, "cells must be in [1, 2^30]");
     ncells *= g.cells[d];
     g.lo[d] = d < dim ? lo_host[d] : 0.0;
-    const double span = d < dim ? hi_host[d] - lo_host[d] : 1.0;
+    const double hi = d < dim ? hi_host[d] : 0.0;
+    const double span = hi - g.lo[d];
+    GSP_REQUIRE(std::isfinite(span) && span >= 0, "the bounding box must be finite, lo <= hi");
     g.h[d] = span > 0 ? span / g.cells[d] : 1.0;
     g.inv_h[d] = 1.0 / g.h[d];
+    g.slack[d] = ldexp(fmax(fabs(g.lo[d]), fabs(hi)), -44);
   }
   GSP_REQUIRE(ncells < (int64_t(1) << 31), "too many cells");
   uint32_t *keys = nullptr, *keys_sorted = nullptr;

@@ -7,6 +7,7 @@ construction is vectorised -- the reference's per-vertex Python loops
 fabrication for the filtering path, not part of the timed hot path.
 """
 import ctypes
+import math
 import os
 
 import numpy as np
@@ -137,13 +138,62 @@ def _check_order(p):
     return p
 
 
+def _require_finite(pts):
+    """``ValueError`` unless every coordinate is finite, as cKDTree: a NaN or an infinity has
+    no place in a distance order."""
+    torch = nat.require_cuda()
+    if not bool(torch.isfinite(pts).all()):
+        raise ValueError("data must be finite")
+
+
+# gsp_knn_grid's bounds: cells per axis (so that ring indices stay in int32) and cells per point
+# (so that the cell table stays a few entries per point)
+_GRID_AXIS_CELLS = 2 ** 30
+_GRID_CELLS_PER_POINT = 4
+
+
+def _knn_grid_cells(lo, hi, n, points_per_cell):
+    """Cells per axis of the uniform grid that ``gsp_knn_grid`` lays over the box [lo, hi] of
+    n points.
+
+    Cubic cells of side h hold ``points_per_cell`` points on average: h^m = volume *
+    points_per_cell / n over the m axes whose span reaches h.  An axis thinner than one cell (a
+    line, a plane, all points equal, a spread at rounding level) gets one cell and leaves the
+    volume, so that it cannot shrink the cells of the others; h is recomputed until no axis drops
+    out.  Counts are clipped in float64 before the integer cast: every axis gets 1 .. 2^30 cells,
+    all of them together at most 4 n.
+    """
+    with np.errstate(over="ignore"):
+        span = np.asarray(hi, dtype=np.float64) - np.asarray(lo, dtype=np.float64)
+    if not np.isfinite(span).all():
+        raise ValueError("the range of the coordinates must be finite")
+    if not points_per_cell > 0:
+        raise ValueError("points_per_cell must be positive")
+    cells = np.ones(span.shape)
+    live = span > 0
+    while live.any():
+        # in logarithms: the volume of a thin box can underflow
+        h = np.exp((np.log(span[live]).sum() + np.log(points_per_cell / n)) / live.sum())
+        thin = live & (span < h)
+        if not thin.any():
+            cells[live] = np.minimum(np.floor(span[live] / h), _GRID_AXIS_CELLS)
+            break
+        live &= ~thin
+    cells = cells.astype(np.int64)
+    while math.prod(cells.tolist()) > min(_GRID_CELLS_PER_POINT * n, 2 ** 31 - 1):
+        cells = np.maximum(cells // 2, 1)
+    return cells.astype(np.int32)
+
+
 def knn_device(points, k, device=None, points_per_cell=3.0, p=2):
     """k nearest neighbours of every point (self excluded by index) on the GPU.
 
     Stands in for ``scipy.spatial.KDTree(X).query(X, k + 1, p=p)`` (nngraph.py:213-216):
     returns (nn, dist), both (N, k) CUDA tensors, ascending (distance, id); k <= 32.  Euclidean
     2-D / 3-D clouds are searched on a cell grid (``gsp_knn_grid``), every other dimension and
-    Minkowski order p >= 1 (inf included) exhaustively (``gsp_knn_brute``); both are exact.
+    Minkowski order p >= 1 (inf included) exhaustively (``gsp_knn_brute``); both are exact and
+    give the same lists, bit for bit.  The grid's cells hold ``points_per_cell`` points on average
+    (:func:`_knn_grid_cells`).  ``ValueError`` for a coordinate that is not finite, as cKDTree.
     """
     torch = nat.require_cuda()
     dev = _device_of(device)
@@ -151,20 +201,18 @@ def knn_device(points, k, device=None, points_per_cell=3.0, p=2):
     pts = _device_points(points, dev)
     n, dim = pts.shape
     if p != 2 or dim not in (2, 3):
+        _require_finite(pts)
         nn = torch.empty((n, k), dtype=torch.int32, device=dev)
         dist = torch.empty((n, k), dtype=torch.float64, device=dev)
         with torch.cuda.device(dev):
             nat.call("gsp_knn_brute", nat.i64(n), nat.i32(dim), pts, nat.i32(k), nat.f64(p), nn,
                      dist, nat.stream_ptr(dev))
         return nn, dist
+    # min and max propagate NaN, so a coordinate that is not finite reaches lo or hi, and
+    # _knn_grid_cells refuses the box
     lo = pts.min(dim=0).values.cpu().numpy().astype(np.float64)
     hi = pts.max(dim=0).values.cpu().numpy().astype(np.float64)
-    span = np.maximum(hi - lo, 1e-300)
-    # cubic cells holding ~points_per_cell points on average
-    h = (np.prod(span) * points_per_cell / n) ** (1.0 / dim)
-    cells = np.maximum(np.floor(span / h), 1).astype(np.int32)
-    while np.prod(cells.astype(np.int64)) >= 2 ** 31:
-        cells = np.maximum(cells // 2, 1)
+    cells = _knn_grid_cells(lo, hi, n, points_per_cell)
     nn = torch.empty((n, k), dtype=torch.int32, device=dev)
     dist = torch.empty((n, k), dtype=torch.float64, device=dev)
     with torch.cuda.device(dev):
@@ -197,12 +245,14 @@ def radius_device(points, epsilon, p=2, device=None):
     Row i holds the j != i with ``dist(x_i, x_j) <= epsilon`` in the Minkowski metric of order p,
     sorted by column -- ``KDTree(X).query_ball_point(X, r=epsilon, p=p)`` and the self filter of
     nngraph.py:228-283.  The number of entries is read once; ``ValueError`` when it does not fit
-    int32 CSR offsets or the free device memory, before anything is allocated for them.
+    int32 CSR offsets or the free device memory, before anything is allocated for them, and for a
+    coordinate that is not finite.
     """
     torch = nat.require_cuda()
     dev = _device_of(device)
     p = _check_order(p)
     pts = _device_points(points, dev)
+    _require_finite(pts)
     n, dim = pts.shape
     indptr = torch.empty(n + 1, dtype=torch.int32, device=dev)
     total = torch.zeros(1, dtype=torch.int64, device=dev)
