@@ -215,11 +215,10 @@ inline int grid_for(int64_t count) {
   return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(count, kBlockThreads), 4096));
 }
 
-// Adds `parts` partials of `count` doubles into out (or copies the only one); frees `part`.
-int finish_parts(double* part, int64_t parts, int64_t count, double* out, cudaStream_t st) {
+// Adds `parts` partials of `count` doubles into out (or copies the only one).
+int finish_parts(const double* part, int64_t parts, int64_t count, double* out, cudaStream_t st) {
   reduce_parts_kernel<<<grid_for(count), kBlockThreads, 0, st>>>(count, parts, part, out);
   GSP_LAUNCH_CHECK("block_reduce_parts");
-  GSP_CUDA(cudaFreeAsync(part, st));
   return GSP_OK;
 }
 
@@ -234,8 +233,9 @@ int gram_mt(int64_t n, const T* A, int64_t ka, const T* B, int64_t kb, double* C
                            kMaxParts * (8 / MT) / std::min(ta * tb, kMaxParts * (8 / MT))));
   const int64_t chunk = ceil_div(ceil_div(n, parts), KS) * KS;
   const int64_t used = ceil_div(n, chunk);
-  double* part = C;
-  if (used > 1) GSP_CUDA(cudaMallocAsync((void**)&part, used * ka * kb * sizeof(double), st));
+  Scratch<double> parts_buf(st);
+  if (used > 1) GSP_CUDA(parts_buf.alloc(used * ka * kb));
+  double* part = used > 1 ? parts_buf.get() : C;
   dim3 grid((unsigned)used, (unsigned)ta, (unsigned)tb);
   block_gram_kernel<T, MT><<<grid, kBlockThreads, 0, st>>>(n, A, ka, B, kb, chunk, part);
   GSP_LAUNCH_CHECK("block_gram");
@@ -294,8 +294,9 @@ int block_residual(int64_t n, const T* X, const T* LX, const double* theta, int6
   const int64_t parts = std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 1024), kMaxParts));
   const int64_t chunk = ceil_div(n, parts);
   const int64_t used = ceil_div(n, chunk);
-  double* part = out;
-  if (used > 1) GSP_CUDA(cudaMallocAsync((void**)&part, used * k * sizeof(double), st));
+  Scratch<double> parts_buf(st);
+  if (used > 1) GSP_CUDA(parts_buf.alloc(used * k));
+  double* part = used > 1 ? parts_buf.get() : out;
   block_residual_kernel<T><<<dim3((unsigned)used, (unsigned)cg), kBlockThreads, 0, st>>>(
       n, X, LX, theta, k, chunk, part);
   GSP_LAUNCH_CHECK("block_residual");

@@ -763,16 +763,15 @@ int tile_plan(int64_t n, const int32_t* indptr, int64_t nsig, int nscales, gsp_t
   if (nsig <= 16 && !getenv("GSPB200_TILE_R")) R = std::max(R, warps_default * (128 / (int)nsig));
   const int64_t n_tiles = n / R;
   if (n_tiles < 1) return GSP_OK;
-  int* dmax = nullptr;
-  GSP_CUDA(cudaMallocAsync((void**)&dmax, sizeof(int), st));
-  GSP_CUDA(cudaMemsetAsync(dmax, 0, sizeof(int), st));
+  Scratch<int> dmax(st);
+  GSP_CUDA(dmax.alloc(1));
+  GSP_CUDA(cudaMemsetAsync(dmax.get(), 0, sizeof(int), st));
   const int blocks = (int)std::min<int64_t>(ceil_div(n / 4 + 1, 256), 2048);
-  tile_nnz_max_kernel<<<blocks, 256, 0, st>>>(n, R, indptr, dmax);
+  tile_nnz_max_kernel<<<blocks, 256, 0, st>>>(n, R, indptr, dmax.get());
   GSP_LAUNCH_CHECK("tile_nnz_max");
   int hmax = 0;
-  GSP_CUDA(cudaMemcpyAsync(&hmax, dmax, sizeof(int), cudaMemcpyDeviceToHost, st));
+  GSP_CUDA(cudaMemcpyAsync(&hmax, dmax.get(), sizeof(int), cudaMemcpyDeviceToHost, st));
   GSP_CUDA(cudaStreamSynchronize(st));
-  cudaFreeAsync(dmax, st);
   const int cap = ((hmax + 8 + 31) / 32) * 32;
   int stages = env_int("GSPB200_TILE_S", nscales <= 1 ? 2 : 3);
   const int warps = std::min(16, std::max(1, env_int("GSPB200_TILE_NW", 16)));

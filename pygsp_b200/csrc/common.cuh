@@ -49,6 +49,46 @@ inline int check_cuda(cudaError_t e, const char* what) {
 
 inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
 
+// Stream-ordered device scratch of one C entry point: allocated on `st` by alloc(), freed on
+// `st` when the owner goes out of scope, so every return path releases it.  An owner that is
+// never allocated holds nullptr and frees nothing.
+template <typename T>
+class Scratch {
+ public:
+  explicit Scratch(cudaStream_t st) : st_(st) {}
+  Scratch(const Scratch&) = delete;
+  Scratch& operator=(const Scratch&) = delete;
+  // The status is ignored: a pointer from cudaMallocAsync freed on its own stream can only fail
+  // to free if the context is already broken, and every later call reports that anyway.
+  ~Scratch() {
+    if (p_) (void)cudaFreeAsync(p_, st_);
+  }
+  // count elements of T; call once per owner
+  cudaError_t alloc(size_t count) {
+    void* p = nullptr;
+    const cudaError_t e = cudaMallocAsync(&p, count * sizeof(T), st_);
+    if (e == cudaSuccess) p_ = static_cast<T*>(p);
+    return e;
+  }
+  T* get() const { return p_; }
+
+ private:
+  T* p_ = nullptr;
+  cudaStream_t st_;
+};
+
+// CUB's two-phase protocol: run(nullptr, bytes) sizes the temporary storage, run(tmp, bytes)
+// does the work; `run` is a callable (void* tmp, size_t& bytes) -> cudaError_t.
+template <typename F>
+int cub_temp(const char* what, cudaStream_t st, F&& run) {
+  size_t bytes = 0;
+  int rc = check_cuda(run(nullptr, bytes), what);
+  if (rc != GSP_OK) return rc;
+  Scratch<char> tmp(st);
+  GSP_CUDA(tmp.alloc(std::max<size_t>(bytes, 16)));
+  return check_cuda(run(tmp.get(), bytes), what);
+}
+
 inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
 // number of SMs of the current device (cached per device)

@@ -279,25 +279,15 @@ int vertex_map(int64_t n, int64_t m, const int32_t* v, int32_t* mptr, int32_t* m
   int rc = scan_rows(mptr, n, st);
   if (rc != GSP_OK) return rc;
   // positions sorted by old id; the radix sort is stable, so each old id's positions increase
-  int32_t *pos = nullptr, *keys_out = nullptr;
-  GSP_CUDA(cudaMallocAsync((void**)&pos, sizeof(int32_t) * m, st));
-  GSP_CUDA(cudaMallocAsync((void**)&keys_out, sizeof(int32_t) * m, st));
-  iota_kernel<<<conn_blocks(m), kConnThreads, 0, st>>>(m, pos);
-  cudaError_t e = cudaGetLastError();
-  note_launch(1);
-  size_t bytes = 0;
-  void* tmp = nullptr;
-  if (e == cudaSuccess)
-    e = cub::DeviceRadixSort::SortPairs(nullptr, bytes, v, keys_out, pos, mpos, (int)m, 0,
-                                        key_bits(n), st);
-  if (e == cudaSuccess) e = cudaMallocAsync(&tmp, bytes ? bytes : 16, st);
-  if (e == cudaSuccess)
-    e = cub::DeviceRadixSort::SortPairs(tmp, bytes, v, keys_out, pos, mpos, (int)m, 0,
-                                        key_bits(n), st);
-  if (tmp) cudaFreeAsync(tmp, st);
-  cudaFreeAsync(pos, st);
-  cudaFreeAsync(keys_out, st);
-  return check_cuda(e, "vertex_map");
+  Scratch<int32_t> pos(st), keys_out(st);
+  GSP_CUDA(pos.alloc(m));
+  GSP_CUDA(keys_out.alloc(m));
+  iota_kernel<<<conn_blocks(m), kConnThreads, 0, st>>>(m, pos.get());
+  GSP_LAUNCH_CHECK("iota");
+  return cub_temp("cub::DeviceRadixSort::SortPairs", st, [&](void* tmp, size_t& bytes) {
+    return cub::DeviceRadixSort::SortPairs(tmp, bytes, v, keys_out.get(), pos.get(), mpos, (int)m,
+                                           0, key_bits(n), st);
+  });
 }
 
 int subgraph_count(int64_t m, const int32_t* indptr, const int32_t* indices, const int32_t* v,
@@ -329,37 +319,26 @@ int component_order(int64_t n, const int32_t* labels, int32_t* perm, int32_t* co
     if (n_components) GSP_CUDA(cudaMemsetAsync(n_components, 0, sizeof(int64_t), st));
     return GSP_OK;
   }
-  int32_t *ids = nullptr, *sorted = nullptr, *rank = nullptr;
-  GSP_CUDA(cudaMallocAsync((void**)&ids, sizeof(int32_t) * n, st));
-  GSP_CUDA(cudaMallocAsync((void**)&sorted, sizeof(int32_t) * n, st));
-  GSP_CUDA(cudaMallocAsync((void**)&rank, sizeof(int32_t) * (n + 1), st));
-  iota_kernel<<<conn_blocks(n), kConnThreads, 0, st>>>(n, ids);
-  root_flags_kernel<<<conn_blocks(n), kConnThreads, 0, st>>>(n, labels, rank);
-  cudaError_t e = cudaGetLastError();
-  note_launch(2);
-  size_t bytes = 0;
-  void* tmp = nullptr;
+  Scratch<int32_t> ids(st), sorted(st), rank(st);
+  GSP_CUDA(ids.alloc(n));
+  GSP_CUDA(sorted.alloc(n));
+  GSP_CUDA(rank.alloc(n + 1));
+  iota_kernel<<<conn_blocks(n), kConnThreads, 0, st>>>(n, ids.get());
+  GSP_LAUNCH_CHECK("iota");
+  root_flags_kernel<<<conn_blocks(n), kConnThreads, 0, st>>>(n, labels, rank.get());
+  GSP_LAUNCH_CHECK("root_flags");
   // vertices by (label, id): a stable sort of the labels
-  if (e == cudaSuccess)
-    e = cub::DeviceRadixSort::SortPairs(nullptr, bytes, labels, sorted, ids, perm, (int)n, 0,
-                                        key_bits(n), st);
-  if (e == cudaSuccess) e = cudaMallocAsync(&tmp, bytes ? bytes : 16, st);
-  if (e == cudaSuccess)
-    e = cub::DeviceRadixSort::SortPairs(tmp, bytes, labels, sorted, ids, perm, (int)n, 0,
-                                        key_bits(n), st);
-  int rc = e == cudaSuccess ? scan_rows(rank, n, st) : GSP_OK;
-  if (e == cudaSuccess && rc == GSP_OK) {
-    component_starts_kernel<<<conn_blocks(n), kConnThreads, 0, st>>>(n, sorted, rank, comp_ptr,
-                                                                     n_components);
-    e = cudaGetLastError();
-    note_launch(1);
-  }
-  if (tmp) cudaFreeAsync(tmp, st);
-  cudaFreeAsync(ids, st);
-  cudaFreeAsync(sorted, st);
-  cudaFreeAsync(rank, st);
+  int rc = cub_temp("cub::DeviceRadixSort::SortPairs", st, [&](void* tmp, size_t& bytes) {
+    return cub::DeviceRadixSort::SortPairs(tmp, bytes, labels, sorted.get(), ids.get(), perm,
+                                           (int)n, 0, key_bits(n), st);
+  });
   if (rc != GSP_OK) return rc;
-  return check_cuda(e, "component_order");
+  rc = scan_rows(rank.get(), n, st);
+  if (rc != GSP_OK) return rc;
+  component_starts_kernel<<<conn_blocks(n), kConnThreads, 0, st>>>(n, sorted.get(), rank.get(),
+                                                                   comp_ptr, n_components);
+  GSP_LAUNCH_CHECK("component_starts");
+  return GSP_OK;
 }
 
 template <typename T>

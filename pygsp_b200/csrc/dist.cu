@@ -155,11 +155,9 @@ int cheby_op_dist(const gsp_dist_plan* p, const gsp_tile_plan* tile, double lmax
     // forward recurrence, reference order (approximations.py:99-112).  With a row
     // permutation the accumulators live in local order in stream-ordered scratch and are
     // scattered to the caller's order at the end.
-    T* r_out = r;
-    if (perm && n > 0) {
-      GSP_CUDA(cudaMallocAsync((void**)&r, sizeof(T) * size_t(nscales) * n * nsig, st));
-    }
-    s.r = r;
+    Scratch<T> local(st);
+    if (perm && n > 0) GSP_CUDA(local.alloc(size_t(nscales) * n * nsig));
+    s.r = local.get() ? local.get() : r;
     int cur = 0, old = 1;
     for (int k = 1; k <= K; ++k) {
       forward_coefs(s, k, m, nscales, lmax, c, ck, c0);
@@ -167,15 +165,14 @@ int cheby_op_dist(const gsp_dist_plan* p, const gsp_tile_plan* tile, double lmax
       s.x_old = s.first ? nullptr : buf[old];
       s.x_new = buf[old];
       rc = dist_step<T>(p, tile, fusable, s, old, base + 1 + k, base + 2 + k, k < K, stream);
-      if (rc != GSP_OK) { if (r != r_out) cudaFreeAsync(r, st); return rc; }
+      if (rc != GSP_OK) return rc;
       trace.mark();
       std::swap(cur, old);
     }
-    if (r != r_out) {
+    if (local.get()) {
       for (int i = 0; i < nscales && rc == GSP_OK; ++i)
-        rc = move_rows<T>(true, n, perm, r + int64_t(i) * n * nsig, nsig, r_out + int64_t(i) * n * nsig,
-                          st);
-      cudaFreeAsync(r, st);
+        rc = move_rows<T>(true, n, perm, local.get() + int64_t(i) * n * nsig, nsig,
+                          r + int64_t(i) * n * nsig, st);
     }
     return rc;
   }

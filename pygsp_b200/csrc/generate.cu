@@ -20,17 +20,6 @@ namespace gsp {
 constexpr int kGenThreads = 256;
 constexpr int kMaxK = 32;
 
-static int scan_inplace(int32_t* indptr, int64_t n, cudaStream_t st) {
-  if (n == 0) return GSP_OK;
-  size_t bytes = 0;
-  GSP_CUDA(cub::DeviceScan::InclusiveSum(nullptr, bytes, indptr + 1, indptr + 1, (int)n, st));
-  void* tmp = nullptr;
-  GSP_CUDA(cudaMallocAsync(&tmp, bytes ? bytes : 16, st));
-  cudaError_t e = cub::DeviceScan::InclusiveSum(tmp, bytes, indptr + 1, indptr + 1, (int)n, st);
-  cudaFreeAsync(tmp, st);
-  return check_cuda(e, "cub::DeviceScan::InclusiveSum");
-}
-
 // --------------------------------------------------------------------- Grid2d
 __global__ void grid2d_count_kernel(int64_t n1, int64_t n2, int32_t* indptr) {
   const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -229,7 +218,7 @@ int gsp_grid2d_count(int64_t n1, int64_t n2, int32_t* indptr, void* stream) {
   cudaStream_t st = gsp::as_stream(stream);
   gsp::grid2d_count_kernel<<<gsp::blocks_for(n1 * n2), gsp::kGenThreads, 0, st>>>(n1, n2, indptr);
   GSP_LAUNCH_CHECK("grid2d_count");
-  return gsp::scan_inplace(indptr, n1 * n2, st);
+  return gsp::scan_rows(indptr, n1 * n2, st);
 }
 
 int gsp_grid2d_fill_f32(int64_t n1, int64_t n2, const int32_t* indptr, int32_t* indices,
@@ -272,41 +261,36 @@ int gsp_knn_grid(int64_t n, int dim, const double* points, int k, const double* 
     g.slack[d] = ldexp(fmax(fabs(g.lo[d]), fabs(hi)), -44);
   }
   GSP_REQUIRE(ncells < (int64_t(1) << 31), "too many cells");
-  uint32_t *keys = nullptr, *keys_sorted = nullptr;
-  int32_t *ids = nullptr, *ids_sorted = nullptr, *cell_start = nullptr;
-  double* sorted_pts = nullptr;
-  GSP_CUDA(cudaMallocAsync((void**)&keys, 4 * n, st));
-  GSP_CUDA(cudaMallocAsync((void**)&keys_sorted, 4 * n, st));
-  GSP_CUDA(cudaMallocAsync((void**)&ids, 4 * n, st));
-  GSP_CUDA(cudaMallocAsync((void**)&ids_sorted, 4 * n, st));
-  GSP_CUDA(cudaMallocAsync((void**)&cell_start, 4 * (ncells + 1), st));
-  GSP_CUDA(cudaMallocAsync((void**)&sorted_pts, 8 * n * dim, st));
+  gsp::Scratch<uint32_t> keys(st), keys_sorted(st);
+  gsp::Scratch<int32_t> ids(st), ids_sorted(st), cell_start(st);
+  gsp::Scratch<double> sorted_pts(st);
+  GSP_CUDA(keys.alloc(n));
+  GSP_CUDA(keys_sorted.alloc(n));
+  GSP_CUDA(ids.alloc(n));
+  GSP_CUDA(ids_sorted.alloc(n));
+  GSP_CUDA(cell_start.alloc(ncells + 1));
+  GSP_CUDA(sorted_pts.alloc(n * dim));
   const int nb = gsp::blocks_for(n);
-  gsp::knn_cell_keys_kernel<<<nb, gsp::kGenThreads, 0, st>>>(n, points, g, keys, ids);
+  gsp::knn_cell_keys_kernel<<<nb, gsp::kGenThreads, 0, st>>>(n, points, g, keys.get(), ids.get());
+  GSP_LAUNCH_CHECK("knn_cell_keys");
   int bits = 1;
   while ((int64_t(1) << bits) < ncells) ++bits;
-  size_t bytes = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, bytes, keys, keys_sorted, ids, ids_sorted, (int)n, 0,
-                                  bits, st);
-  void* tmp = nullptr;
-  GSP_CUDA(cudaMallocAsync(&tmp, bytes ? bytes : 16, st));
-  cudaError_t e = cub::DeviceRadixSort::SortPairs(tmp, bytes, keys, keys_sorted, ids, ids_sorted,
-                                                  (int)n, 0, bits, st);
-  if (e == cudaSuccess) {
-    gsp::knn_cell_start_kernel<<<gsp::blocks_for(ncells + 1), gsp::kGenThreads, 0, st>>>(
-        n, ncells, keys_sorted, cell_start);
-    gsp::knn_gather_points_kernel<<<nb, gsp::kGenThreads, 0, st>>>(n, dim, points, ids_sorted,
-                                                                  sorted_pts);
-    gsp::knn_query_kernel<<<nb, gsp::kGenThreads, 0, st>>>(n, k, g, sorted_pts, ids_sorted,
-                                                          cell_start, nn_idx, nn_dist);
-    gsp::note_launch(3);
-    e = cudaGetLastError();
-  }
-  cudaFreeAsync(tmp, st);
-  cudaFreeAsync(keys, st); cudaFreeAsync(keys_sorted, st);
-  cudaFreeAsync(ids, st); cudaFreeAsync(ids_sorted, st);
-  cudaFreeAsync(cell_start, st); cudaFreeAsync(sorted_pts, st);
-  return gsp::check_cuda(e, "gsp_knn_grid");
+  const int rc = gsp::cub_temp("cub::DeviceRadixSort::SortPairs", st, [&](void* tmp, size_t& b) {
+    return cub::DeviceRadixSort::SortPairs(tmp, b, keys.get(), keys_sorted.get(), ids.get(),
+                                           ids_sorted.get(), (int)n, 0, bits, st);
+  });
+  if (rc != GSP_OK) return rc;
+  gsp::knn_cell_start_kernel<<<gsp::blocks_for(ncells + 1), gsp::kGenThreads, 0, st>>>(
+      n, ncells, keys_sorted.get(), cell_start.get());
+  GSP_LAUNCH_CHECK("knn_cell_start");
+  gsp::knn_gather_points_kernel<<<nb, gsp::kGenThreads, 0, st>>>(n, dim, points, ids_sorted.get(),
+                                                                sorted_pts.get());
+  GSP_LAUNCH_CHECK("knn_gather_points");
+  gsp::knn_query_kernel<<<nb, gsp::kGenThreads, 0, st>>>(n, k, g, sorted_pts.get(),
+                                                        ids_sorted.get(), cell_start.get(), nn_idx,
+                                                        nn_dist);
+  GSP_LAUNCH_CHECK("knn_query");
+  return GSP_OK;
 }
 
 int gsp_knn_to_csr_f32(int64_t n, int k, const int32_t* nn_idx, const double* nn_dist,

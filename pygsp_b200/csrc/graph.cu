@@ -46,13 +46,9 @@ __device__ __forceinline__ double warp_max(double v) {
 int scan_rows(int32_t* indptr, int64_t n, cudaStream_t st) {
   // indptr[0] = 0 and indptr[1..n] hold row sizes on entry
   if (n == 0) return GSP_OK;
-  size_t bytes = 0;
-  GSP_CUDA(cub::DeviceScan::InclusiveSum(nullptr, bytes, indptr + 1, indptr + 1, (int)n, st));
-  void* tmp = nullptr;
-  GSP_CUDA(cudaMallocAsync(&tmp, bytes ? bytes : 16, st));
-  cudaError_t e = cub::DeviceScan::InclusiveSum(tmp, bytes, indptr + 1, indptr + 1, (int)n, st);
-  cudaFreeAsync(tmp, st);
-  return check_cuda(e, "cub::DeviceScan::InclusiveSum");
+  return cub_temp("cub::DeviceScan::InclusiveSum", st, [&](void* tmp, size_t& bytes) {
+    return cub::DeviceScan::InclusiveSum(tmp, bytes, indptr + 1, indptr + 1, (int)n, st);
+  });
 }
 
 // ---- adjacency inspection (graph.py:111-128) --------------------------------
@@ -156,28 +152,21 @@ static int csr_transpose(int64_t n, int64_t nnz, const int32_t* indptr, const in
                          cudaStream_t st) {
   GSP_CUDA(cudaMemsetAsync(t_indptr, 0, sizeof(int32_t) * (n + 1), st));
   if (n == 0 || nnz == 0) return GSP_OK;
-  uint64_t *keys_in = nullptr, *keys_out = nullptr;
-  GSP_CUDA(cudaMallocAsync((void**)&keys_in, sizeof(uint64_t) * nnz, st));
-  GSP_CUDA(cudaMallocAsync((void**)&keys_out, sizeof(uint64_t) * nnz, st));
-  transpose_keys_kernel<T><<<row_blocks(n), kRowThreads, 0, st>>>(n, indptr, indices, keys_in,
-                                                                   t_indptr);
+  Scratch<uint64_t> keys_in(st), keys_out(st);
+  GSP_CUDA(keys_in.alloc(nnz));
+  GSP_CUDA(keys_out.alloc(nnz));
+  transpose_keys_kernel<T><<<row_blocks(n), kRowThreads, 0, st>>>(n, indptr, indices,
+                                                                   keys_in.get(), t_indptr);
+  GSP_LAUNCH_CHECK("transpose_keys");
   int bits = 33;
   while ((int64_t(1) << (bits - 32)) < n && bits < 64) ++bits;
-  size_t bytes = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, bytes, keys_in, keys_out, data, t_data, (int)nnz, 0,
-                                  bits, st);
-  void* tmp = nullptr;
-  GSP_CUDA(cudaMallocAsync(&tmp, bytes ? bytes : 16, st));
-  cudaError_t e = cub::DeviceRadixSort::SortPairs(tmp, bytes, keys_in, keys_out, data, t_data,
-                                                  (int)nnz, 0, bits, st);
-  if (e == cudaSuccess) {
-    transpose_unpack_kernel<<<(int)ceil_div(nnz, 256), 256, 0, st>>>(nnz, keys_out, t_indices);
-    e = cudaGetLastError();
-  }
-  cudaFreeAsync(tmp, st);
-  cudaFreeAsync(keys_in, st);
-  cudaFreeAsync(keys_out, st);
-  if (e != cudaSuccess) return check_cuda(e, "csr_transpose");
+  int rc = cub_temp("cub::DeviceRadixSort::SortPairs", st, [&](void* tmp, size_t& bytes) {
+    return cub::DeviceRadixSort::SortPairs(tmp, bytes, keys_in.get(), keys_out.get(), data, t_data,
+                                           (int)nnz, 0, bits, st);
+  });
+  if (rc != GSP_OK) return rc;
+  transpose_unpack_kernel<<<(int)ceil_div(nnz, 256), 256, 0, st>>>(nnz, keys_out.get(), t_indices);
+  GSP_LAUNCH_CHECK("transpose_unpack");
   return scan_rows(t_indptr, n, st);
 }
 
@@ -210,41 +199,37 @@ static int coo_to_csr(int64_t n, int64_t nnz, const int32_t* rows, const int32_t
   GSP_CUDA(cudaMemsetAsync(indptr, 0, sizeof(int32_t) * (n + 1), st));
   *n_unique_out = 0;
   if (nnz == 0) return GSP_OK;
-  uint64_t *k0 = nullptr, *k1 = nullptr, *ku = nullptr;
-  T* v1 = nullptr;
-  int* scal = nullptr;       // [0] bad indices, [1] number of unique keys
-  GSP_CUDA(cudaMallocAsync((void**)&k0, 8 * nnz, st));
-  GSP_CUDA(cudaMallocAsync((void**)&k1, 8 * nnz, st));
-  GSP_CUDA(cudaMallocAsync((void**)&ku, 8 * nnz, st));
-  GSP_CUDA(cudaMallocAsync((void**)&v1, sizeof(T) * nnz, st));
-  GSP_CUDA(cudaMallocAsync((void**)&scal, 2 * sizeof(int), st));
-  GSP_CUDA(cudaMemsetAsync(scal, 0, 2 * sizeof(int), st));
-  const int nb = (int)ceil_div(nnz, 256);
-  coo_keys_kernel<<<nb, 256, 0, st>>>(nnz, rows, cols, n, k0, scal);
+  Scratch<uint64_t> k0(st), k1(st), ku(st);
+  Scratch<T> v1(st);
+  Scratch<int> scal(st);     // [0] bad indices, [1] number of unique keys
+  GSP_CUDA(k0.alloc(nnz));
+  GSP_CUDA(k1.alloc(nnz));
+  GSP_CUDA(ku.alloc(nnz));
+  GSP_CUDA(v1.alloc(nnz));
+  GSP_CUDA(scal.alloc(2));
+  GSP_CUDA(cudaMemsetAsync(scal.get(), 0, 2 * sizeof(int), st));
+  coo_keys_kernel<<<(int)ceil_div(nnz, 256), 256, 0, st>>>(nnz, rows, cols, n, k0.get(),
+                                                           scal.get());
+  GSP_LAUNCH_CHECK("coo_keys");
   int bits = 33;
   while ((int64_t(1) << (bits - 32)) < n && bits < 64) ++bits;
-  size_t b1 = 0, b2 = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, b1, k0, k1, vals, v1, (int)nnz, 0, bits, st);
-  cub::DeviceReduce::ReduceByKey(nullptr, b2, k1, ku, v1, data, scal + 1, cub::Sum(), (int)nnz, st);
-  void* tmp = nullptr;
-  const size_t bytes = std::max(b1, b2);
-  GSP_CUDA(cudaMallocAsync(&tmp, bytes ? bytes : 16, st));
-  cudaError_t e = cub::DeviceRadixSort::SortPairs(tmp, b1, k0, k1, vals, v1, (int)nnz, 0, bits, st);
-  if (e == cudaSuccess)
-    e = cub::DeviceReduce::ReduceByKey(tmp, b2, k1, ku, v1, data, scal + 1, cub::Sum(), (int)nnz, st);
+  int rc = cub_temp("cub::DeviceRadixSort::SortPairs", st, [&](void* tmp, size_t& bytes) {
+    return cub::DeviceRadixSort::SortPairs(tmp, bytes, k0.get(), k1.get(), vals, v1.get(),
+                                           (int)nnz, 0, bits, st);
+  });
+  if (rc != GSP_OK) return rc;
+  rc = cub_temp("cub::DeviceReduce::ReduceByKey", st, [&](void* tmp, size_t& bytes) {
+    return cub::DeviceReduce::ReduceByKey(tmp, bytes, k1.get(), ku.get(), v1.get(), data,
+                                          scal.get() + 1, cub::Sum(), (int)nnz, st);
+  });
+  if (rc != GSP_OK) return rc;
   int host[2] = {0, 0};
-  if (e == cudaSuccess) e = cudaMemcpyAsync(host, scal, sizeof(host), cudaMemcpyDeviceToHost, st);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-  if (e == cudaSuccess && host[0] == 0) {
-    coo_unpack_kernel<<<(int)ceil_div(host[1] > 0 ? host[1] : 1, 256), 256, 0, st>>>(host[1], ku,
-                                                                                    indices, indptr);
-    e = cudaGetLastError();
-    note_launch(2);
-  }
-  cudaFreeAsync(tmp, st); cudaFreeAsync(k0, st); cudaFreeAsync(k1, st); cudaFreeAsync(ku, st);
-  cudaFreeAsync(v1, st); cudaFreeAsync(scal, st);
-  if (e != cudaSuccess) return check_cuda(e, "coo_to_csr");
+  GSP_CUDA(cudaMemcpyAsync(host, scal.get(), sizeof(host), cudaMemcpyDeviceToHost, st));
+  GSP_CUDA(cudaStreamSynchronize(st));
   if (host[0] != 0) return fail(GSP_ERR_ARG, "COO index out of range (%s)", "rows/cols");
+  coo_unpack_kernel<<<(int)ceil_div(host[1] > 0 ? host[1] : 1, 256), 256, 0, st>>>(
+      host[1], ku.get(), indices, indptr);
+  GSP_LAUNCH_CHECK("coo_unpack");
   *n_unique_out = host[1];
   return scan_rows(indptr, n, st);
 }

@@ -318,65 +318,59 @@ int krylov_basis(int64_t n, int64_t ncols, const int32_t* indptr, const int32_t*
   const int64_t plane = n * ns;
   // scratch: partials (P.used x order x ns), h (order x ns), ss, den, scale (ns), ||A||_inf
   const int64_t n_part = P.used * order * ns, n_h = int64_t(order) * ns;
-  double* scratch = nullptr;
-  GSP_CUDA(cudaMallocAsync((void**)&scratch, (n_part + n_h + 3 * ns + 1) * sizeof(double), st));
-  double *part = scratch, *h = part + n_part, *ss = h + n_h, *den = ss + ns, *scale = den + ns;
-  double* anorm = scale + ns;
-  int rc = GSP_OK;
+  Scratch<double> scratch(st);
+  GSP_CUDA(scratch.alloc(n_part + n_h + 3 * ns + 1));
+  double *part = scratch.get(), *h = part + n_part, *ss = h + n_h, *den = ss + ns;
+  double *scale = den + ns, *anorm = scale + ns;
   const dim3 red((unsigned)P.used, (unsigned)cg);
   const double tol = kBreakdown * Eps<T>::value;
-  do {
-    if ((rc = check_cuda(cudaMemsetAsync(anorm, 0, sizeof(double), st), "memset")) != GSP_OK) break;
-    krylov_norm_bound_kernel<T><<<grid_for(n), kThreads, 0, st>>>(
-        n, indptr, data, reinterpret_cast<unsigned long long*>(anorm));
-    note_launch(1);
-    krylov_sumsq_kernel<T><<<red, kThreads, 0, st>>>(n, x, ns, P.chunk, part);
-    note_launch(1);
-    if ((rc = reduce(part, P.used, ns, ss, st)) != GSP_OK) break;
-    krylov_start_kernel<<<grid_for(ns), kThreads, 0, st>>>(ns, ss, beta, m, den, scale);
-    krylov_scale_kernel<T><<<grid_for(plane), kThreads, 0, st>>>(plane, ns, x, den, V);
-    note_launch(2);
-    if ((rc = check_cuda(cudaGetLastError(), "krylov_start")) != GSP_OK) break;
-    for (int k = 0; k < order && rc == GSP_OK; ++k) {
-      const T* q = V + k * plane;
-      T* r = V + (k + 1) * plane;
-      if ((rc = spmm(n, indptr, indices, data, q, ns, r, st)) != GSP_OK) break;
-      krylov_three_term_kernel<T><<<red, kThreads, 0, st>>>(
-          n, r, q, k ? q - plane : nullptr, beta + int64_t(k) * ns, ns, P.chunk, part);
-      note_launch(1);
-      if ((rc = reduce(part, P.used, ns, alpha + int64_t(k) * ns, st)) != GSP_OK) break;
-      if (k == order - 1) break;           // beta_order and q_order are not part of the result
-      krylov_axpy_kernel<T><<<red, kThreads, 0, st>>>(n, r, q, alpha + int64_t(k) * ns, ns,
-                                                      P.chunk, k == 0, part);
-      note_launch(1);
-      if (k > 0) {                         // full reorthogonalisation, as approximations.py:335
-        const int64_t kb = k + 1;
-        krylov_cgs_gram_kernel<T><<<dim3((unsigned)P.used, (unsigned)cg,
-                                         (unsigned)ceil_div(kb, kGramTile)),
-                                    kThreads, 0, st>>>(n, V, kb, r, ns, P.chunk, part);
-        note_launch(1);
-        if ((rc = reduce(part, P.used, kb * ns, h, st)) != GSP_OK) break;
-        krylov_cgs_update_kernel<T><<<red, kThreads, 0, st>>>(n, V, kb, h, r, ns, P.chunk, part);
-        note_launch(1);
-      }
-      if ((rc = reduce(part, P.used, ns, ss, st)) != GSP_OK) break;
-      krylov_step_kernel<<<grid_for(ns), kThreads, 0, st>>>(
-          ns, k, tol, anorm, alpha + int64_t(k) * ns, ss, beta + int64_t(k + 1) * ns, m, den, scale);
-      krylov_scale_kernel<T><<<grid_for(plane), kThreads, 0, st>>>(plane, ns, r, den, r);
-      note_launch(2);
-      rc = check_cuda(cudaGetLastError(), "krylov_step");
+  GSP_CUDA(cudaMemsetAsync(anorm, 0, sizeof(double), st));
+  krylov_norm_bound_kernel<T><<<grid_for(n), kThreads, 0, st>>>(
+      n, indptr, data, reinterpret_cast<unsigned long long*>(anorm));
+  GSP_LAUNCH_CHECK("krylov_norm_bound");
+  krylov_sumsq_kernel<T><<<red, kThreads, 0, st>>>(n, x, ns, P.chunk, part);
+  GSP_LAUNCH_CHECK("krylov_sumsq");
+  int rc = reduce(part, P.used, ns, ss, st);
+  if (rc != GSP_OK) return rc;
+  krylov_start_kernel<<<grid_for(ns), kThreads, 0, st>>>(ns, ss, beta, m, den, scale);
+  GSP_LAUNCH_CHECK("krylov_start");
+  krylov_scale_kernel<T><<<grid_for(plane), kThreads, 0, st>>>(plane, ns, x, den, V);
+  GSP_LAUNCH_CHECK("krylov_scale");
+  for (int k = 0; k < order; ++k) {
+    const T* q = V + k * plane;
+    T* r = V + (k + 1) * plane;
+    if ((rc = spmm(n, indptr, indices, data, q, ns, r, st)) != GSP_OK) return rc;
+    krylov_three_term_kernel<T><<<red, kThreads, 0, st>>>(
+        n, r, q, k ? q - plane : nullptr, beta + int64_t(k) * ns, ns, P.chunk, part);
+    GSP_LAUNCH_CHECK("krylov_three_term");
+    if ((rc = reduce(part, P.used, ns, alpha + int64_t(k) * ns, st)) != GSP_OK) return rc;
+    if (k == order - 1) break;             // beta_order and q_order are not part of the result
+    krylov_axpy_kernel<T><<<red, kThreads, 0, st>>>(n, r, q, alpha + int64_t(k) * ns, ns,
+                                                    P.chunk, k == 0, part);
+    GSP_LAUNCH_CHECK("krylov_axpy");
+    if (k > 0) {                           // full reorthogonalisation, as approximations.py:335
+      const int64_t kb = k + 1;
+      krylov_cgs_gram_kernel<T><<<dim3((unsigned)P.used, (unsigned)cg,
+                                       (unsigned)ceil_div(kb, kGramTile)),
+                                  kThreads, 0, st>>>(n, V, kb, r, ns, P.chunk, part);
+      GSP_LAUNCH_CHECK("krylov_cgs_gram");
+      if ((rc = reduce(part, P.used, kb * ns, h, st)) != GSP_OK) return rc;
+      krylov_cgs_update_kernel<T><<<red, kThreads, 0, st>>>(n, V, kb, h, r, ns, P.chunk, part);
+      GSP_LAUNCH_CHECK("krylov_cgs_update");
     }
-    if (rc != GSP_OK) break;
-    // V^T s, computed explicitly as the reference does (approximations.py:274)
-    krylov_cgs_gram_kernel<T><<<dim3((unsigned)P.used, (unsigned)cg,
-                                     (unsigned)ceil_div(order, kGramTile)),
-                                kThreads, 0, st>>>(n, V, order, x, ns, P.chunk, part);
-    note_launch(1);
-    if ((rc = reduce(part, P.used, int64_t(order) * ns, vs, st)) != GSP_OK) break;
-    rc = check_cuda(cudaGetLastError(), "krylov_basis");
-  } while (false);
-  const int frc = check_cuda(cudaFreeAsync(scratch, st), "cudaFreeAsync");
-  return rc != GSP_OK ? rc : frc;
+    if ((rc = reduce(part, P.used, ns, ss, st)) != GSP_OK) return rc;
+    krylov_step_kernel<<<grid_for(ns), kThreads, 0, st>>>(
+        ns, k, tol, anorm, alpha + int64_t(k) * ns, ss, beta + int64_t(k + 1) * ns, m, den, scale);
+    GSP_LAUNCH_CHECK("krylov_step");
+    krylov_scale_kernel<T><<<grid_for(plane), kThreads, 0, st>>>(plane, ns, r, den, r);
+    GSP_LAUNCH_CHECK("krylov_scale");
+  }
+  // V^T s, computed explicitly as the reference does (approximations.py:274)
+  krylov_cgs_gram_kernel<T><<<dim3((unsigned)P.used, (unsigned)cg,
+                                   (unsigned)ceil_div(order, kGramTile)),
+                              kThreads, 0, st>>>(n, V, order, x, ns, P.chunk, part);
+  GSP_LAUNCH_CHECK("krylov_cgs_gram");
+  return reduce(part, P.used, int64_t(order) * ns, vs, st);
 }
 
 template <typename T>

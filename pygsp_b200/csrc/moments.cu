@@ -269,20 +269,15 @@ int moments_step(int64_t n, const T* tn, const T* tc, int64_t b, int m, int k, d
   GSP_REQUIRE(n >= 1 && b >= 1 && m >= 1 && k >= 0 && k < m, "bad sizes");
   GSP_REQUIRE(ceil_div(b, 32) < 65536, "block too wide");
   const Parts P = row_parts(n);
-  double* part = nullptr;
-  GSP_CUDA(cudaMallocAsync((void**)&part, P.used * 2 * b * sizeof(double), st));
+  Scratch<double> part(st);
+  GSP_CUDA(part.alloc(P.used * 2 * b));
   moments_part_kernel<T><<<dim3((unsigned)P.used, (unsigned)ceil_div(b, 32)), kThreads, 0, st>>>(
-      n, tn, tc, b, P.chunk, part);
-  note_launch(1);
-  int rc = check_cuda(cudaGetLastError(), "moments_part");
-  if (rc == GSP_OK) {
-    moments_reduce_kernel<<<grid_for(2 * b), kThreads, 0, st>>>(2 * b, P.used, part,
-                                                                 sums + int64_t(k) * 2 * b);
-    note_launch(1);
-    rc = check_cuda(cudaGetLastError(), "moments_reduce");
-  }
-  const int frc = check_cuda(cudaFreeAsync(part, st), "cudaFreeAsync");
-  return rc != GSP_OK ? rc : frc;
+      n, tn, tc, b, P.chunk, part.get());
+  GSP_LAUNCH_CHECK("moments_part");
+  moments_reduce_kernel<<<grid_for(2 * b), kThreads, 0, st>>>(2 * b, P.used, part.get(),
+                                                               sums + int64_t(k) * 2 * b);
+  GSP_LAUNCH_CHECK("moments_reduce");
+  return GSP_OK;
 }
 
 template <typename T>
@@ -291,104 +286,82 @@ int two_hop_count(int64_t n, const int32_t* indptr, const int32_t* indices, cons
   GSP_REQUIRE(n >= 0 && n < (int64_t(1) << 31), "bad sizes");
   if (n == 0) return GSP_OK;
   // scratch: cand (n), heavy ids' candidate counts (n), heavy ids (n), counter
-  char* scratch = nullptr;
-  const size_t bytes = size_t(n) * (8 + 8 + 4) + 8;
-  GSP_CUDA(cudaMallocAsync((void**)&scratch, bytes, st));
-  int64_t* cand = reinterpret_cast<int64_t*>(scratch);
+  Scratch<char> scratch(st);
+  GSP_CUDA(scratch.alloc(size_t(n) * (8 + 8 + 4) + 8));
+  int64_t* cand = reinterpret_cast<int64_t*>(scratch.get());
   int64_t* ids_cand = cand + n;
   unsigned long long* counter = reinterpret_cast<unsigned long long*>(ids_cand + n);
   int32_t* ids = reinterpret_cast<int32_t*>(counter + 1);
-  int32_t* table = nullptr;
-  int64_t* meta = nullptr;
-  int rc = GSP_OK;
-  do {
-    two_hop_degree_kernel<T><<<grid_for(n), kThreads, 0, st>>>(n, indptr, data, degree);
-    two_hop_cand_kernel<T><<<grid_for(n * 32), kThreads, 0, st>>>(n, indptr, indices, data,
-                                                                   degree, cand);
-    two_hop_light_kernel<T><<<(unsigned)std::min<int64_t>(ceil_div(n, kLightWarps), 65535),
-                              kLightWarps * 32, 0, st>>>(n, indptr, indices, data, cand, two_hop);
-    note_launch(3);
-    if ((rc = check_cuda(cudaGetLastError(), "two_hop_light")) != GSP_OK) break;
-    if ((rc = check_cuda(cudaMemsetAsync(counter, 0, 8, st), "memset")) != GSP_OK) break;
-    two_hop_select_kernel<<<grid_for(n), kThreads, 0, st>>>(n, cand, ids, ids_cand, counter);
-    note_launch(1);
-    unsigned long long heavy = 0;
-    if ((rc = check_cuda(cudaMemcpyAsync(&heavy, counter, 8, cudaMemcpyDeviceToHost, st),
-                         "heavy count")) != GSP_OK)
-      break;
-    if ((rc = check_cuda(cudaStreamSynchronize(st), "two_hop sync")) != GSP_OK) break;
-    if (heavy == 0) break;
-    std::vector<int32_t> hid(heavy);
-    std::vector<int64_t> hc(heavy);
-    if ((rc = check_cuda(cudaMemcpyAsync(hid.data(), ids, heavy * 4, cudaMemcpyDeviceToHost, st),
-                         "heavy ids")) != GSP_OK ||
-        (rc = check_cuda(cudaMemcpyAsync(hc.data(), ids_cand, heavy * 8, cudaMemcpyDeviceToHost,
-                                         st), "heavy counts")) != GSP_OK ||
-        (rc = check_cuda(cudaStreamSynchronize(st), "two_hop sync")) != GSP_OK)
-      break;
-    // process the heavy rows in increasing id order (the selection's order is not fixed)
-    std::vector<size_t> order(heavy);
-    for (size_t q = 0; q < heavy; ++q) order[q] = q;
-    std::sort(order.begin(), order.end(), [&](size_t a, size_t c) { return hid[a] < hid[c]; });
-    std::vector<int64_t> size(heavy);
-    int64_t widest = 0;
-    for (size_t q = 0; q < heavy; ++q) {
-      int64_t s = 1;
-      while (s < 2 * hc[q]) s <<= 1;
-      size[q] = s;
-      widest = std::max(widest, s);
+  two_hop_degree_kernel<T><<<grid_for(n), kThreads, 0, st>>>(n, indptr, data, degree);
+  GSP_LAUNCH_CHECK("two_hop_degree");
+  two_hop_cand_kernel<T><<<grid_for(n * 32), kThreads, 0, st>>>(n, indptr, indices, data, degree,
+                                                                 cand);
+  GSP_LAUNCH_CHECK("two_hop_cand");
+  two_hop_light_kernel<T><<<(unsigned)std::min<int64_t>(ceil_div(n, kLightWarps), 65535),
+                            kLightWarps * 32, 0, st>>>(n, indptr, indices, data, cand, two_hop);
+  GSP_LAUNCH_CHECK("two_hop_light");
+  GSP_CUDA(cudaMemsetAsync(counter, 0, 8, st));
+  two_hop_select_kernel<<<grid_for(n), kThreads, 0, st>>>(n, cand, ids, ids_cand, counter);
+  GSP_LAUNCH_CHECK("two_hop_select");
+  unsigned long long heavy = 0;
+  GSP_CUDA(cudaMemcpyAsync(&heavy, counter, 8, cudaMemcpyDeviceToHost, st));
+  GSP_CUDA(cudaStreamSynchronize(st));
+  if (heavy == 0) return GSP_OK;
+  std::vector<int32_t> hid(heavy);
+  std::vector<int64_t> hc(heavy);
+  GSP_CUDA(cudaMemcpyAsync(hid.data(), ids, heavy * 4, cudaMemcpyDeviceToHost, st));
+  GSP_CUDA(cudaMemcpyAsync(hc.data(), ids_cand, heavy * 8, cudaMemcpyDeviceToHost, st));
+  GSP_CUDA(cudaStreamSynchronize(st));
+  // process the heavy rows in increasing id order (the selection's order is not fixed)
+  std::vector<size_t> order(heavy);
+  for (size_t q = 0; q < heavy; ++q) order[q] = q;
+  std::sort(order.begin(), order.end(), [&](size_t a, size_t c) { return hid[a] < hid[c]; });
+  std::vector<int64_t> size(heavy);
+  int64_t widest = 0;
+  for (size_t q = 0; q < heavy; ++q) {
+    int64_t s = 1;
+    while (s < 2 * hc[q]) s <<= 1;
+    size[q] = s;
+    widest = std::max(widest, s);
+  }
+  const int64_t budget = std::max(kHeavySlots, widest);
+  const int64_t max_rows = 65535;
+  Scratch<int32_t> table(st);
+  Scratch<int64_t> meta(st);
+  GSP_CUDA(table.alloc(budget));
+  GSP_CUDA(meta.alloc(max_rows * 3));
+  int64_t* d_offs = meta.get();
+  int64_t* d_sizes = d_offs + max_rows;
+  int32_t* d_rows = reinterpret_cast<int32_t*>(d_offs + 2 * max_rows);
+  std::vector<int32_t> rows;
+  std::vector<int64_t> offs, sizes;
+  for (size_t q0 = 0; q0 < heavy;) {
+    rows.clear();
+    offs.clear();
+    sizes.clear();
+    int64_t used = 0;
+    size_t q = q0;
+    for (; q < heavy && int64_t(rows.size()) < max_rows; ++q) {
+      const size_t o = order[q];
+      if (used + size[o] > budget) break;
+      rows.push_back(hid[o]);
+      offs.push_back(used);
+      sizes.push_back(size[o]);
+      used += size[o];
     }
-    const int64_t budget = std::max(kHeavySlots, widest);
-    const int64_t max_rows = 65535;
-    if ((rc = check_cuda(cudaMallocAsync((void**)&table, budget * sizeof(int32_t), st),
-                         "cudaMallocAsync")) != GSP_OK)
-      break;
-    if ((rc = check_cuda(cudaMallocAsync((void**)&meta, max_rows * 3 * sizeof(int64_t), st),
-                         "cudaMallocAsync")) != GSP_OK)
-      break;
-    int64_t* d_offs = meta;
-    int64_t* d_sizes = meta + max_rows;
-    int32_t* d_rows = reinterpret_cast<int32_t*>(meta + 2 * max_rows);
-    std::vector<int32_t> rows;
-    std::vector<int64_t> offs, sizes;
-    for (size_t q0 = 0; q0 < heavy && rc == GSP_OK;) {
-      rows.clear();
-      offs.clear();
-      sizes.clear();
-      int64_t used = 0;
-      size_t q = q0;
-      for (; q < heavy && int64_t(rows.size()) < max_rows; ++q) {
-        const size_t o = order[q];
-        if (used + size[o] > budget) break;
-        rows.push_back(hid[o]);
-        offs.push_back(used);
-        sizes.push_back(size[o]);
-        used += size[o];
-      }
-      q0 = q;
-      const size_t nr = rows.size();
-      // the host vectors must outlive the copies: synchronise before the next chunk refills them
-      if ((rc = check_cuda(cudaMemsetAsync(table, 0xFF, used * sizeof(int32_t), st), "memset")) != GSP_OK ||
-          (rc = check_cuda(cudaMemcpyAsync(d_rows, rows.data(), nr * 4, cudaMemcpyHostToDevice, st),
-                           "rows")) != GSP_OK ||
-          (rc = check_cuda(cudaMemcpyAsync(d_offs, offs.data(), nr * 8, cudaMemcpyHostToDevice, st),
-                           "offs")) != GSP_OK ||
-          (rc = check_cuda(cudaMemcpyAsync(d_sizes, sizes.data(), nr * 8, cudaMemcpyHostToDevice,
-                                           st), "sizes")) != GSP_OK)
-        break;
-      two_hop_heavy_kernel<T><<<dim3(kHeavySlices, (unsigned)nr), kThreads, 0, st>>>(
-          indptr, indices, data, d_rows, d_offs, d_sizes, table, two_hop);
-      note_launch(1);
-      if ((rc = check_cuda(cudaGetLastError(), "two_hop_heavy")) != GSP_OK) break;
-      rc = check_cuda(cudaStreamSynchronize(st), "two_hop sync");
-    }
-  } while (false);
-  int frc = GSP_OK;
-  if (table) frc = check_cuda(cudaFreeAsync(table, st), "cudaFreeAsync");
-  if (meta && frc == GSP_OK) frc = check_cuda(cudaFreeAsync(meta, st), "cudaFreeAsync");
-  const int frc2 = check_cuda(cudaFreeAsync(scratch, st), "cudaFreeAsync");
-  if (rc != GSP_OK) return rc;
-  return frc != GSP_OK ? frc : frc2;
+    q0 = q;
+    const size_t nr = rows.size();
+    // the host vectors must outlive the copies: synchronise before the next chunk refills them
+    GSP_CUDA(cudaMemsetAsync(table.get(), 0xFF, used * sizeof(int32_t), st));
+    GSP_CUDA(cudaMemcpyAsync(d_rows, rows.data(), nr * 4, cudaMemcpyHostToDevice, st));
+    GSP_CUDA(cudaMemcpyAsync(d_offs, offs.data(), nr * 8, cudaMemcpyHostToDevice, st));
+    GSP_CUDA(cudaMemcpyAsync(d_sizes, sizes.data(), nr * 8, cudaMemcpyHostToDevice, st));
+    two_hop_heavy_kernel<T><<<dim3(kHeavySlices, (unsigned)nr), kThreads, 0, st>>>(
+        indptr, indices, data, d_rows, d_offs, d_sizes, table.get(), two_hop);
+    GSP_LAUNCH_CHECK("two_hop_heavy");
+    GSP_CUDA(cudaStreamSynchronize(st));
+  }
+  return GSP_OK;
 }
 
 }  // namespace

@@ -250,24 +250,18 @@ int sparsify_sample(int64_t ne, const uint64_t* weights, int64_t q, uint64_t see
                     int64_t* counts, cudaStream_t st) {
   GSP_CUDA(cudaMemsetAsync(counts, 0, sizeof(int64_t) * ne, st));
   if (ne == 0 || q == 0) return GSP_OK;
-  unsigned long long* cum = nullptr;
-  GSP_CUDA(cudaMallocAsync((void**)&cum, sizeof(uint64_t) * ne, st));
+  Scratch<unsigned long long> cum(st);
+  GSP_CUDA(cum.alloc(ne));
   const unsigned long long* w = reinterpret_cast<const unsigned long long*>(weights);
-  size_t bytes = 0;
-  void* tmp = nullptr;
-  cudaError_t e = cub::DeviceScan::InclusiveSum(nullptr, bytes, w, cum, (int)ne, st);
-  if (e == cudaSuccess) e = cudaMallocAsync(&tmp, bytes ? bytes : 16, st);
-  if (e == cudaSuccess) e = cub::DeviceScan::InclusiveSum(tmp, bytes, w, cum, (int)ne, st);
-  if (e == cudaSuccess) {
-    const int64_t chunks = ceil_div(q, kDrawsPerChunk);
-    sample_kernel<<<(int)ceil_div(chunks, kSampleThreads), kSampleThreads, 0, st>>>(
-        ne, cum, q, seed, reinterpret_cast<unsigned long long*>(counts));
-    e = cudaGetLastError();
-    note_launch(1);
-  }
-  if (tmp) cudaFreeAsync(tmp, st);
-  cudaFreeAsync(cum, st);
-  return check_cuda(e, "sparsify_sample");
+  const int rc = cub_temp("cub::DeviceScan::InclusiveSum", st, [&](void* tmp, size_t& bytes) {
+    return cub::DeviceScan::InclusiveSum(tmp, bytes, w, cum.get(), (int)ne, st);
+  });
+  if (rc != GSP_OK) return rc;
+  const int64_t chunks = ceil_div(q, kDrawsPerChunk);
+  sample_kernel<<<(int)ceil_div(chunks, kSampleThreads), kSampleThreads, 0, st>>>(
+      ne, cum.get(), q, seed, reinterpret_cast<unsigned long long*>(counts));
+  GSP_LAUNCH_CHECK("sparsify_sample");
+  return GSP_OK;
 }
 
 }  // namespace gsp
