@@ -548,6 +548,35 @@ int gsp_radius_fill_f64(int64_t n, int d, const double* points, double epsilon, 
 GSPB200_DECLARE_NEIGHBOR_API(f32, float)
 GSPB200_DECLARE_NEIGHBOR_API(f64, double)
 
+/* ---------------------------------------------------------------- spring layout ---
+ * Fruchterman-Reingold force-directed layout of pygsp/graphs/_layout.py:169-219 on the device,
+ * in float64 whatever the type of W (csrc/layout.cu).  pos / pos_in / pos_out / states are
+ * (n, dim) row-major double blocks; W is canonical CSR (n x n) and only its entries with w > 0
+ * attract (the reference's A = W > 0, graph.py:718, row i of a directed W); fixed (n bytes, may
+ * be NULL) marks vertices that do not move but still repel (_layout.py:198).  One iteration:
+ *   disp_i = sum_j delta_ij k^2 / d_ij^2 - sum_{j : w_ij > 0} delta_ij d_ij / k,
+ *   delta_ij = p_i - p_j, d_ij = max(|delta_ij|, 0.01),           (_layout.py:200-211)
+ *   p_i += disp_i t / length_i, length_i = |disp_i|, 0.1 if < 0.01  (_layout.py:212-215).
+ * The sums run in a fixed order that depends on n only: results are bit-identical from run to
+ * run and from card to card, and differ from the reference's order by rounding.
+ * gsp_spring_step_*:   one iteration at temperature t from pos_in into pos_out (distinct
+ *     blocks).
+ * gsp_spring_layout_*: `iterations` iterations (_layout.py:194-217) from the start in pos, at
+ *     temperatures temps_host[0 .. iterations) (host array; the caller's cooling schedule,
+ *     _layout.py:190-191, 217); the final positions are written back to pos.  states (may be
+ *     NULL; iterations x n x dim) receives the positions after every iteration.
+ */
+#define GSPB200_DECLARE_LAYOUT_API(SUF, T)                                                       \
+  int gsp_spring_step_##SUF(int64_t n, int dim, const int32_t* indptr, const int32_t* indices,   \
+                            const T* data, double k, double t, const uint8_t* fixed,             \
+                            const double* pos_in, double* pos_out, void* stream);                \
+  int gsp_spring_layout_##SUF(int64_t n, int dim, const int32_t* indptr, const int32_t* indices, \
+                              const T* data, double k, int iterations, const double* temps_host, \
+                              const uint8_t* fixed, double* pos, double* states, void* stream);
+
+GSPB200_DECLARE_LAYOUT_API(f32, float)
+GSPB200_DECLARE_LAYOUT_API(f64, double)
+
 #define GSPB200_DECLARE_GRAPH_API(SUF, T)                                                        \
   int gsp_csr_inspect_##SUF(int64_t n, const int32_t* indptr, const int32_t* indices,            \
                             const T* data, int64_t* stats_dev, void* stream);                    \

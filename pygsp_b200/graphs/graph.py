@@ -8,11 +8,12 @@ _get_upper_bound, :368-405 is_directed), through ``FourierMixIn``
 (graphs/difference.py) of the differential operator, ``get_edge_list`` and
 ``dirichlet_energy``, and through ``ConnectivityMixIn`` (graphs/connectivity.py) of
 ``is_connected``, ``extract_components``, ``subgraph``, ``set_signal`` and
-``is_weighted``.  Same constructor signature, same attributes, same
+``is_weighted``, and through ``LayoutMixIn`` (graphs/layout.py) of ``set_coordinates``.  Same
+constructor signature, same attributes, same
 exceptions and log messages; the adjacency, the Laplacian and every vector
 derived from them live on the GPU and are produced by the kernels of
 ``libgspb200`` (csrc/graph.cu, csrc/lanczos.cu, csrc/difference.cu,
-csrc/connectivity.cu).  Out of
+csrc/connectivity.cu, csrc/layout.cu).  Out of
 scope here, as in SURVEY.md section 2: plotting, IO.
 """
 import numpy as np
@@ -24,11 +25,12 @@ from .connectivity import ConnectivityMixIn
 from .csr import DeviceCSR
 from .difference import DifferenceMixIn
 from .fourier import FourierMixIn
+from .layout import LayoutMixIn
 
 _LAP = {"combinatorial": 0, "normalized": 1}
 
 
-class Graph(FourierMixIn, DifferenceMixIn, ConnectivityMixIn):
+class Graph(FourierMixIn, DifferenceMixIn, ConnectivityMixIn, LayoutMixIn):
     r"""Graph defined by a (weighted) adjacency matrix.
 
     Parameters
