@@ -281,6 +281,46 @@ GSPB200_DECLARE_CG_API(f64, double)
 GSPB200_DECLARE_FB_API(f32, float)
 GSPB200_DECLARE_FB_API(f64, double)
 
+/* Graph total variation prox, min_z 1/2 ||x - z||^2 + gamma ||D^T A z||_1, by FISTA on the dual
+ * (csrc/tv.cu): pygsp/optimization.py:24-103 (prox_tv), which hands the problem to pyunlocbox's
+ * norm_l1 prox (:100-103) and cannot run as written.  D is the (n x n_edges) differential operator
+ * and Dt its transpose (csrc/difference.cu: two entries per Dt row, none for a self-loop).
+ * Blocks are row-major with nsig columns.  The caller owns the state and zero-fills it before
+ * iteration 0: U2 holds two dual blocks of max(n, n_edges) rows (u_k is block k % 2; the rows
+ * past n_edges stay zero), G one (n_edges, nsig) block (g_k = D^T A z_k), scal_dev
+ * GSPB200_TV_HISTORY + 2 cap doubles: [0] t_k, [1] the stop criterion (0 = running, 1 rtol,
+ * 2 maxit), [2] the stop iteration, then P_k = 1/2 ||x - z_k||^2 + gamma ||g_k||_1 at
+ * GSPB200_TV_HISTORY + 2 k and gap_k = gamma sum(|g_k| - u_k g_k) at GSPB200_TV_HISTORY + 2 k + 1
+ * (appending zeros between calls grows cap).
+ * Stop rule on k >= 1 (optimization.py:53-57): |P_k - P_{k-1}| < tol |P_k|, or
+ * P_k = P_{k-1} = 0 with tol > 0 (rtol); k >= maxit (maxit, checked second).  Once it holds the
+ * edge passes do nothing, so u_k of the stopping iteration stays in U2; z does not (see
+ * gsp_prox_tv_primal_*).  tau is the dual step 1 / (gamma nu_bar), nu_bar >= ||D^T A||^2.
+ * gsp_prox_tv_*: iterations [it0, it1) of the A = identity path (it1 <= cap), each a vertex pass
+ *     z = x - gamma D u_k (replaces l1_at, :89-90 / :97-98) and an edge pass.
+ * gsp_prox_tv_edges_*: the edge pass of iteration it alone, for an A given by the caller: forms
+ *     g_k = D^T w from w = A z_k (replaces l1_a, :86-87 / :94-95), z = z_k enters the objective.
+ * gsp_prox_tv_primal_*: z = x - gamma D u for one dual block u of max(n, n_edges) rows: the
+ *     vertex pass of gsp_prox_tv_*, bit for bit (z_k of the stopping iteration from u_k). */
+#define GSPB200_TV_HISTORY 3080
+#define GSPB200_DECLARE_TV_API(SUF, T)                                                           \
+  int gsp_prox_tv_##SUF(int64_t n, int64_t n_edges, int64_t d_nnz, const int32_t* d_indptr,     \
+                        const int32_t* d_indices, const T* d_data, const int32_t* dt_indptr,    \
+                        const int32_t* dt_indices, const T* dt_data, const T* x, int64_t nsig,  \
+                        double gamma, double tau, double tol, int maxit, T* z, T* U2, T* G,     \
+                        int it0, int it1, int cap, double* scal_dev, void* stream);             \
+  int gsp_prox_tv_edges_##SUF(int64_t n, int64_t n_edges, const int32_t* dt_indptr,             \
+                              const int32_t* dt_indices, const T* dt_data, const T* w,          \
+                              const T* x, const T* z, int64_t nsig, double gamma, double tau,   \
+                              double tol, int maxit, T* U2, T* G, int it, int cap,              \
+                              double* scal_dev, void* stream);                                  \
+  int gsp_prox_tv_primal_##SUF(int64_t n, int64_t d_nnz, const int32_t* d_indptr,               \
+                               const int32_t* d_indices, const T* d_data, const T* x,           \
+                               int64_t nsig, double gamma, const T* u, T* z, void* stream);
+
+GSPB200_DECLARE_TV_API(f32, float)
+GSPB200_DECLARE_TV_API(f64, double)
+
 /* --------------------------------------------------------- spectral basis ---
  * Tall-skinny block kernels of the graph Fourier basis (pygsp_b200/graphs/fourier.py): gft /
  * igft and the partial eigensolver that stands for scipy's eigsh (Chebyshev-filtered subspace

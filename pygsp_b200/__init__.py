@@ -12,6 +12,7 @@ from . import filters  # noqa: F401
 from . import reduction  # noqa: F401
 from . import learning  # noqa: F401
 from . import features  # noqa: F401
+from . import optimization  # noqa: F401
 
 __version__ = "0.1.0"
 

@@ -19,6 +19,7 @@
 // The one-hot Y is never formed: label[row] is the class of a labelled vertex, -1 otherwise.
 #include <math.h>
 
+#include "reduce.cuh"
 #include "step.cuh"
 
 namespace gsp {
@@ -37,18 +38,6 @@ struct FbStop {
   double atol, dtol, rtol, xtol;   // NaN = off (every comparison with NaN is false)
   int maxit;                       // < 0 = off
 };
-
-static inline int fb_blocks(int64_t n, int rpb) {
-  return (int)std::max<int64_t>(
-      1, std::min<int64_t>(ceil_div(n, rpb), std::min<int64_t>(int64_t(sm_count()) * 4, kFbMaxBlocks)));
-}
-
-// sum over the w lanes of an aligned power-of-two sub-warp (xor butterfly: fixed order)
-template <typename S>
-__device__ __forceinline__ S group_sum(S v, int w) {
-  for (int off = w >> 1; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
-  return v;
-}
 
 template <typename T>
 __global__ void __launch_bounds__(kFbThreads)
@@ -226,7 +215,7 @@ int fb_simplex_run(int64_t n, int64_t nnz, const int32_t* indptr, const int32_t*
     w = 32;
     while (32 * V < C) V *= 2;
   }
-  const int blocks = fb_blocks(n, kFbThreads / w);
+  const int blocks = pass_blocks(n, kFbThreads / w, kFbMaxBlocks);
   const int64_t nc = n * C;
   if (it0 == 0) {
     const int ib = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(nc, kFbThreads),
