@@ -22,6 +22,7 @@ tests); the compute is the same C-ABI step kernel as the single-GPU path.
 import numpy as np
 
 from . import _native as nat
+from .graphs.csr import row_ids
 
 
 def even_bounds(n, parts):
@@ -133,7 +134,7 @@ class HaloPlan:
         owner = np.searchsorted(bounds, self.halo_ids, side="right") - 1
         self.recv_counts = np.bincount(owner, minlength=P).astype(np.int64)
         self.n_halo = int(self.halo_ids.size)
-        row_of = torch.repeat_interleave(torch.arange(n_local, device=dev), counts)
+        row_of = row_ids(indptr)
         is_boundary = torch.zeros(n_local, dtype=torch.bool, device=dev)
         is_boundary[row_of[~owned]] = True
         boundary = torch.nonzero(is_boundary).flatten()
@@ -458,8 +459,7 @@ class PartitionedCheby:
         p = self.plan
         n = p.n_local
         dev = self.device
-        ptr = self.indptr.long()
-        row_of = torch.repeat_interleave(torch.arange(n, device=dev), ptr[1:] - ptr[:-1])
+        row_of = row_ids(self.indptr)
         idx, val = self.indices.long(), self.data.double()
         on_diag = idx == row_of
         dw = torch.zeros(n, dtype=torch.float64, device=dev)

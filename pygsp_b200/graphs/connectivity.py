@@ -14,7 +14,7 @@ does the work in HBM:
   batch.
 * ``subgraph`` builds ``W[vertices, :][:, vertices]`` by count -> scan -> fill through a
   multiplicity map of the kept vertices; rows come out sorted when ``vertices`` is strictly
-  increasing, otherwise they are sorted by ``gsp_coo_to_csr_*``.
+  increasing, otherwise they are sorted by ``DeviceCSR.from_coo`` (graphs/csr.py).
 * ``extract_components`` labels the components of ``W > 0`` (a negative edge does not join two
   components, as in the reference), orders the vertices by (component, id) and builds ONE
   block-diagonal CSR; component k is a slice of it.  Only the vertex ids of ``orig_idx`` and
@@ -142,48 +142,6 @@ class ConnectivityMixIn:
                 bad - n if bad < 0 else bad, n))
         return a, torch.from_numpy(a.astype(np.int32)).to(self.device)
 
-    def _induced(self, v, labels=None, increasing=False):
-        """W[v, :][:, v] as a canonical DeviceCSR (m x m) for device int32 ids v; with labels,
-        only the entries whose two ends carry the same label are kept.  ``increasing``: v is
-        strictly increasing, or lists the vertices by (label, id) with labels given, so that
-        the rows come out sorted."""
-        torch = nat.require_cuda()
-        W, n, m = self._adjacency, self.n_vertices, int(v.numel())
-        dev = self.device
-        if m == 0:
-            return DeviceCSR(torch.zeros(1, dtype=torch.int32, device=dev),
-                             torch.empty(0, dtype=torch.int32, device=dev),
-                             torch.empty(0, dtype=self.dtype, device=dev), (0, 0))
-        mptr = torch.empty(n + 1, dtype=torch.int32, device=dev)
-        mpos = torch.empty(m, dtype=torch.int32, device=dev)
-        s_indptr = torch.empty(m + 1, dtype=torch.int32, device=dev)
-        nnz = torch.empty(1, dtype=torch.int64, device=dev)
-        with torch.cuda.device(dev):
-            nat.call("gsp_vertex_map", nat.i64(n), nat.i64(m), v, mptr, mpos, self._stream())
-            nat.call("gsp_subgraph_count", nat.i64(m), W.indptr, W.indices, v, mptr, labels,
-                     s_indptr, nnz, self._stream())
-        nnz = int(nnz.item())
-        if nnz >= 2 ** 31:
-            raise ValueError("The subgraph would have {} entries; at most 2^31 - 1 are "
-                             "supported.".format(nnz))
-        s_indices = torch.empty(nnz, dtype=torch.int32, device=dev)
-        s_data = torch.empty(nnz, dtype=self.dtype, device=dev)
-        rows = None if increasing else torch.empty(nnz, dtype=torch.int32, device=dev)
-        self._call("gsp_subgraph_fill", nat.i64(m), W.indptr, W.indices, W.data, v, mptr, mpos,
-                   labels, s_indptr, s_indices, s_data, rows)
-        if rows is None or nnz == 0:
-            return DeviceCSR(s_indptr, s_indices, s_data, (m, m))
-        # repeated or unordered vertices: sort each row (no two entries coincide)
-        import ctypes
-        indptr = torch.empty(m + 1, dtype=torch.int32, device=dev)
-        indices = torch.empty(nnz, dtype=torch.int32, device=dev)
-        data = torch.empty(nnz, dtype=self.dtype, device=dev)
-        uniq = ctypes.c_int64(0)
-        self._call("gsp_coo_to_csr", nat.i64(m), nat.i64(nnz), rows, s_indices, s_data, indptr,
-                    indices, data, ctypes.byref(uniq))
-        assert uniq.value == nnz, (uniq.value, nnz)
-        return DeviceCSR(indptr, indices, data, (m, m))
-
     def _child(self, W, ids_host, ids_dev):
         """Graph on W with the coords, plotting, Laplacian type and signals of the vertices
         ids of this graph (graph.py:248-255), in this graph's dtype and on its device."""
@@ -219,7 +177,10 @@ class ConnectivityMixIn:
             increasing = bool(np.all(ids_host[1:] > ids_host[:-1]))
         else:
             increasing = v.numel() < 2 or bool(torch.all(v[1:] > v[:-1]))
-        return self._child(self._induced(v, None, increasing), ids_host, v)
+        W, rows = self._adjacency.induced(v, None, increasing)
+        if rows is not None:        # repeated or unordered vertices: sort each row
+            W = DeviceCSR.from_coo(rows, W.indices, W.data, W.shape)
+        return self._child(W, ids_host, v)
 
     def extract_components(self):
         r"""Split the graph into connected components (graph.py:444-508).
@@ -244,7 +205,7 @@ class ConnectivityMixIn:
             nat.call("gsp_component_order", nat.i64(n), labels, perm, comp_ptr, n_components,
                      self._stream())
         # one block-diagonal CSR: component k is rows / columns [ptr[k], ptr[k+1])
-        S = self._induced(perm, labels, increasing=True)
+        S, _ = self._adjacency.induced(perm, labels, increasing=True)
         ptr = comp_ptr[:int(n_components.item()) + 1]
         offsets = S.indptr[ptr.long()].cpu().numpy()
         ptr = ptr.cpu().numpy()

@@ -1,15 +1,28 @@
 """CSR matrix resident in HBM: int32 indptr / indices + float32|float64 data.
 
 This is what ``Graph.W`` and ``Graph.L`` are in this engine (the reference
-holds ``scipy.sparse.csr_matrix`` objects, graph.py:109,620).  It offers the
-small read-only surface the filtering path and its callers use: ``shape``,
-``nnz``, ``dot``, ``toarray``, ``diagonal``, plus ``to_scipy`` to leave the
-device.  The differential operator ``G.D`` is one too, (N, Ne), with its
-transpose attached as ``.T`` by the builder (graphs/difference.py).
+holds ``scipy.sparse.csr_matrix`` objects, graph.py:109,620).  Besides the
+read-only surface of the filtering path (``shape``, ``nnz``, ``dot``,
+``toarray``, ``diagonal``, ``to_scipy``), this module owns every device
+operation that builds or reshapes CSR structure: assembly from COO triplets
+(``from_coo``), ``transpose``, ``symmetrize``, ``eliminate_zeros``, induced
+submatrices (``induced``), the row id of every entry (:func:`row_ids`) and
+the dense float64 copy (``to_dense``).  The differential operator ``G.D`` is
+one too, (N, Ne), with its transpose attached as ``.T`` by the builder
+(graphs/difference.py).
 """
 import numpy as np
 
 from .. import _native as nat
+
+_SYMMETRIZE_MODES = {"maximum": 0, "fill": 1, "tril": 2, "triu": 3}
+
+
+def row_ids(indptr):
+    """Row id (int64) of every entry of the CSR structure ``indptr``, on its device."""
+    import torch
+    counts = (indptr[1:] - indptr[:-1]).long()
+    return torch.repeat_interleave(torch.arange(indptr.numel() - 1, device=indptr.device), counts)
 
 
 class DeviceCSR:
@@ -76,6 +89,123 @@ class DeviceCSR:
         data = torch.from_numpy(np.ascontiguousarray(M.data)).to(device=device, dtype=dtype)
         return cls(indptr, indices, data, M.shape)
 
+    @classmethod
+    def from_coo(cls, rows, cols, vals, shape):
+        """Canonical CSR of COO triplets in HBM: what ``sparse.csr_matrix(coo)`` does at
+        graph.py:109 -- sort by (row, col), sum duplicates in emission order -- on the device
+        (``gsp_coo_to_csr_*``).  Integer rows / cols, float32 or float64 vals; the result lives
+        on vals' device.  ``ValueError`` for 2^31 triplets or more, before anything is touched."""
+        nnz = int(vals.numel())
+        if nnz >= 2 ** 31:
+            raise ValueError("The result would have {} entries; at most 2^31 - 1 are "
+                             "supported.".format(nnz))
+        import ctypes
+        torch = nat.require_cuda()
+        dev, n = vals.device, int(shape[0])
+        indptr = torch.empty(n + 1, dtype=torch.int32, device=dev)
+        indices = torch.empty(nnz, dtype=torch.int32, device=dev)
+        data = torch.empty(nnz, dtype=vals.dtype, device=dev)
+        uniq = ctypes.c_int64(0)
+        with torch.cuda.device(dev):
+            nat.call("gsp_coo_to_csr_" + nat.suffix(vals.dtype), nat.i64(n), nat.i64(nnz),
+                     rows.to(dev, torch.int32).contiguous(), cols.to(dev, torch.int32).contiguous(),
+                     vals.contiguous(), indptr, indices, data, ctypes.byref(uniq),
+                     nat.stream_ptr(dev))
+        m = int(uniq.value)
+        return cls(indptr, indices[:m].contiguous(), data[:m].contiguous(), shape)
+
+    def _call(self, name, *args):
+        """Native entry point ``name`` on this matrix's device and its current stream."""
+        torch = nat.require_cuda()
+        with torch.cuda.device(self.device):
+            nat.call(name, *args, nat.stream_ptr(self.device))
+
+    def _empty(self, nnz):
+        """(indices, data) buffers of nnz entries on this matrix's device and in its dtype."""
+        torch = nat.require_cuda()
+        return (torch.empty(nnz, dtype=torch.int32, device=self.device),
+                torch.empty(nnz, dtype=self.dtype, device=self.device))
+
+    # -- reshaping ------------------------------------------------------------------
+    def transpose(self):
+        """M^T of a square matrix as sorted CSR (``gsp_csr_transpose_*``)."""
+        torch = nat.require_cuda()
+        n = self.shape[0]
+        tp = torch.empty(n + 1, dtype=torch.int32, device=self.device)
+        ti, td = self._empty(self.nnz)
+        self._call("gsp_csr_transpose_" + nat.suffix(self.dtype), nat.i64(n), nat.i64(self.nnz),
+                   self.indptr, self.indices, self.data, tp, ti, td)
+        return DeviceCSR(tp, ti, td, self.shape)
+
+    def symmetrize(self, method="average", transpose=None):
+        """utils.symmetrize(M, method) of a square matrix, on the device (utils.py:244-277).
+
+        Each row of M is merged with the same row of M^T (``transpose``, when the caller has it
+        already): 'average' is (M + M^T)/2 (``gsp_csr_average_*``); 'maximum', 'fill', 'tril' and
+        'triu' go through ``gsp_csr_symmetrize_*``.  The reference's arithmetic, so values are
+        bit-equal to SciPy's in float64.  Exact zeros are dropped."""
+        if self.shape[0] != self.shape[1]:
+            raise ValueError("Matrix must be square.")
+        if method == "average":
+            name, mode = "gsp_csr_average_", ()
+        elif method in _SYMMETRIZE_MODES:
+            name, mode = "gsp_csr_symmetrize_", (nat.i32(_SYMMETRIZE_MODES[method]),)
+        else:
+            raise ValueError("Unknown symmetrization method {}.".format(method))
+        torch = nat.require_cuda()
+        n, sfx = self.shape[0], nat.suffix(self.dtype)
+        T = self.transpose() if transpose is None else transpose
+        operands = (self.indptr, self.indices, self.data, T.indptr, T.indices, T.data)
+        sp = torch.empty(n + 1, dtype=torch.int32, device=self.device)
+        self._call(name + "count_" + sfx, nat.i64(n), *mode, *operands, sp)
+        si, sd = self._empty(int(sp[-1].item()) if n else 0)
+        self._call(name + "fill_" + sfx, nat.i64(n), *mode, *operands, sp, si, sd)
+        return DeviceCSR(sp, si, sd, self.shape)
+
+    def eliminate_zeros(self):
+        """M without its stored zeros (graph.py:128), by the compaction kernels."""
+        torch = nat.require_cuda()
+        n, sfx = self.shape[0], nat.suffix(self.dtype)
+        indptr = torch.empty(n + 1, dtype=torch.int32, device=self.device)
+        self._call("gsp_csr_compact_count_" + sfx, nat.i64(n), self.indptr, self.data, indptr)
+        indices, data = self._empty(int(indptr[-1].item()) if n else 0)
+        self._call("gsp_csr_compact_fill_" + sfx, nat.i64(n), self.indptr, self.indices, self.data,
+                   indptr, indices, data)
+        return DeviceCSR(indptr, indices, data, self.shape)
+
+    def induced(self, v, labels=None, increasing=False):
+        """Entries of M[v, :][:, v] (m x m) for device int32 ids v, by map -> count -> fill.
+
+        With ``labels`` (int32, one per vertex of M) only the entries whose two ends carry the
+        same label are kept.  Returns (S, rows).  ``increasing`` (v strictly increasing, or
+        listing the vertices by (label, id) with labels given): the rows come out sorted, S is
+        canonical and rows is None.  Otherwise each row of S holds its entries in M's column order
+        mapped through v, unsorted, and rows (int32) is the row of every entry, so that
+        ``DeviceCSR.from_coo(rows, S.indices, S.data, S.shape)`` is the canonical matrix.
+        ``ValueError`` when the result would hold 2^31 entries or more."""
+        torch = nat.require_cuda()
+        n, m, dev = self.shape[0], int(v.numel()), self.device
+        if m == 0:
+            S = DeviceCSR(torch.zeros(1, dtype=torch.int32, device=dev), *self._empty(0), (0, 0))
+            return S, None if increasing else S.indices
+        mptr = torch.empty(n + 1, dtype=torch.int32, device=dev)
+        mpos = torch.empty(m, dtype=torch.int32, device=dev)
+        s_indptr = torch.empty(m + 1, dtype=torch.int32, device=dev)
+        nnz = torch.empty(1, dtype=torch.int64, device=dev)
+        self._call("gsp_vertex_map", nat.i64(n), nat.i64(m), v, mptr, mpos)
+        self._call("gsp_subgraph_count", nat.i64(m), self.indptr, self.indices, v, mptr, labels,
+                   s_indptr, nnz)
+        nnz = int(nnz.item())
+        if nnz >= 2 ** 31:
+            raise ValueError("The subgraph would have {} entries; at most 2^31 - 1 are "
+                             "supported.".format(nnz))
+        s_indices, s_data = self._empty(nnz)
+        rows = None if increasing else torch.empty(nnz, dtype=torch.int32, device=dev)
+        self._call("gsp_subgraph_fill_" + nat.suffix(self.dtype), nat.i64(m), self.indptr,
+                   self.indices, self.data, v, mptr, mpos, labels, s_indptr, s_indices, s_data,
+                   rows)
+        return DeviceCSR(s_indptr, s_indices, s_data, (m, m)), rows
+
     # -- introspection --------------------------------------------------------
     @property
     def nnz(self):
@@ -93,7 +223,7 @@ class DeviceCSR:
         return "<DeviceCSR {}x{}, nnz={}, {}, {}>".format(
             self.shape[0], self.shape[1], self.nnz, self.data.dtype, self.data.device)
 
-    # -- leaving the device -----------------------------------------------------
+    # -- leaving the device, dense copies ----------------------------------------
     def to_scipy(self):
         from scipy import sparse
         return sparse.csr_matrix((self.data.cpu().numpy(), self.indices.cpu().numpy(),
@@ -111,6 +241,13 @@ class DeviceCSR:
 
     def toarray(self):
         return self.to_scipy().toarray()
+
+    def to_dense(self):
+        """The matrix as a dense float64 tensor on its device."""
+        torch = nat.require_cuda()
+        dense = torch.zeros(self.shape, dtype=torch.float64, device=self.device)
+        dense[row_ids(self.indptr), self.indices.long()] = self.data.double()
+        return dense
 
     def diagonal(self):
         return self.to_scipy().diagonal()

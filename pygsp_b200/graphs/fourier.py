@@ -168,10 +168,7 @@ class FourierMixIn:
                 "of device memory ({2:.1f} GB free). Pass n_eigenvectors to compute a partial "
                 "basis.".format(n, need / 2 ** 30, free / 2 ** 30))
         with torch.cuda.device(self.device):
-            rows = torch.repeat_interleave(torch.arange(n, device=self.device),
-                                           (L.indptr[1:] - L.indptr[:-1]).long())
-            dense = torch.zeros((n, n), dtype=torch.float64, device=self.device)
-            dense[rows, L.indices.long()] = L.data.double()
+            dense = L.to_dense()
             e, U = torch.linalg.eigh(dense)
             del dense
             U = U[:, :k].to(self.dtype).contiguous()
@@ -235,7 +232,7 @@ class FourierMixIn:
             return self._U[:, -1].double().cpu().numpy()
         if n <= DENSE_CROSSOVER:
             with torch.cuda.device(self.device):
-                _, U = torch.linalg.eigh(self._dense_laplacian())
+                _, U = torch.linalg.eigh(self.L.to_dense())
             return U[:, -1].cpu().numpy()
         cap = MAX_ITERATIONS if max_iter is None else int(max_iter)
         tol = 1e-10 if self.dtype == torch.float64 else 1e-5
@@ -258,16 +255,6 @@ class FourierMixIn:
                 return X[:, -1].double().cpu().numpy()
         raise ValueError("The Chebyshev-filtered subspace iteration for the largest eigenvector "
                          "did not converge in {} iterations.".format(cap))
-
-    def _dense_laplacian(self):
-        """L as a dense float64 device matrix."""
-        torch = nat.require_cuda()
-        n, L = self.n_vertices, self.L
-        rows = torch.repeat_interleave(torch.arange(n, device=self.device),
-                                       (L.indptr[1:] - L.indptr[:-1]).long())
-        dense = torch.zeros((n, n), dtype=torch.float64, device=self.device)
-        dense[rows, L.indices.long()] = L.data.double()
-        return dense
 
     def _apply_laplacian(self, X):
         """L X by the recurrence step (alpha = 1, beta = 0): the tiled kernel where it applies."""

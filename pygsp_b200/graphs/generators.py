@@ -6,7 +6,6 @@ construction is vectorised -- the reference's per-vertex Python loops
 (nngraph.py:221-226) make it unusable beyond ~1e6 vertices.  They are input
 fabrication for the filtering path, not part of the timed hot path.
 """
-import ctypes
 import math
 import os
 
@@ -15,8 +14,8 @@ from scipy import sparse, spatial
 
 from .. import _native as nat
 from .. import utils
-from .csr import DeviceCSR
-from .graph import Graph, _torch_dtype, symmetrize_average_device, symmetrize_device
+from .csr import DeviceCSR, row_ids
+from .graph import Graph, _torch_dtype
 
 _DATA = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "data")
 
@@ -227,16 +226,23 @@ def knn_adjacency_device(points, k, sigma=None, dtype=None, device=None):
     torch = nat.require_cuda()
     dev, dt = _device_of(device), _torch_dtype(torch, dtype)
     nn, dist = knn_device(points, k, dev)
-    n = nn.shape[0]
     if sigma is None:
         sigma = float(dist.mean().item())
+    return _knn_gauss_csr(nn, dist, sigma, dt).symmetrize("average"), sigma
+
+
+def _knn_gauss_csr(nn, dist, sigma, dt):
+    """Directed Gaussian k-NN matrix W[i, nn[i]] = exp(-dist[i]^2 / sigma) of (n, k) neighbour
+    lists, sorted rows, in dtype dt on the lists' device (``gsp_knn_to_csr_*``)."""
+    torch = nat.require_cuda()
+    (n, k), dev = nn.shape, nn.device
     indptr = torch.empty(n + 1, dtype=torch.int32, device=dev)
     indices = torch.empty(n * k, dtype=torch.int32, device=dev)
     data = torch.empty(n * k, dtype=dt, device=dev)
     with torch.cuda.device(dev):
         nat.call("gsp_knn_to_csr_" + nat.suffix(dt), nat.i64(n), nat.i32(k), nn, dist,
                  nat.f64(sigma), indptr, indices, data, nat.stream_ptr(dev))
-    return symmetrize_average_device(DeviceCSR(indptr, indices, data, (n, n))), sigma
+    return DeviceCSR(indptr, indices, data, (n, n))
 
 
 def radius_device(points, epsilon, p=2, device=None):
@@ -407,18 +413,11 @@ class NNGraph(Graph):
     def _device_adjacency(self, X, k, sigma, p, epsilon, dtype, device):
         torch = nat.require_cuda()
         dev, dt = _device_of(device), _torch_dtype(torch, dtype)
-        n = X.shape[0]
         if self.NNtype == "knn":     # with 'average': the steps of knn_adjacency_device
             nn, dist = knn_device(X, k, dev, p=p)
             if sigma is None:
                 sigma = float(dist.mean().item())
-            indptr = torch.empty(n + 1, dtype=torch.int32, device=dev)
-            indices = torch.empty(n * k, dtype=torch.int32, device=dev)
-            data = torch.empty(n * k, dtype=dt, device=dev)
-            with torch.cuda.device(dev):
-                nat.call("gsp_knn_to_csr_" + nat.suffix(dt), nat.i64(n), nat.i32(k), nn, dist,
-                         nat.f64(sigma), indptr, indices, data, nat.stream_ptr(dev))
-            W = DeviceCSR(indptr, indices, data, (n, n))
+            W = _knn_gauss_csr(nn, dist, sigma, dt)
         else:
             D = radius_device(X, epsilon, p, dev)
             if sigma is None:
@@ -426,7 +425,7 @@ class NNGraph(Graph):
                     raise ValueError("No neighbors found")
                 sigma = float(D.data.mean().item())
             W = _gauss_weights_device(D, sigma, dt)
-        return symmetrize_device(W, self.symmetrize_type), sigma
+        return W.symmetrize(self.symmetrize_type), sigma
 
     def _host_adjacency(self, X, k, sigma, p, epsilon):
         N = X.shape[0]
@@ -500,7 +499,7 @@ class Grid2dImgPatches(Graph):
 
     ``W = aggregate(Wp, Wg)`` of the :class:`ImgPatches` adjacency Wp and the
     :class:`Grid2d` adjacency Wg.  The default ``Wp + Wg`` is summed on the device (COO
-    concatenation, then ``gsp_coo_to_csr_*``, which adds duplicates); a user-supplied
+    concatenation, then ``DeviceCSR.from_coo``, which adds duplicates); a user-supplied
     ``aggregate`` receives both as SciPy CSR matrices, as in the reference.  Keyword arguments
     go to :class:`ImgPatches`; the graph takes the grid's coordinates.
     """
@@ -513,32 +512,13 @@ class Grid2dImgPatches(Graph):
         self.Gp = ImgPatches(img, **kwargs)
         if aggregate is None:
             Wp, Wg = self.Gp.W, self.Gg.W
-            rows = torch.cat([_csr_rows(Wp), _csr_rows(Wg)])
-            cols = torch.cat([Wp.indices, Wg.indices])
-            vals = torch.cat([Wp.data, Wg.data.to(Wp.dtype)])
-            n = h * w
-            indptr = torch.empty(n + 1, dtype=torch.int32, device=Wp.device)
-            indices = torch.empty(vals.numel(), dtype=torch.int32, device=Wp.device)
-            data = torch.empty(vals.numel(), dtype=Wp.dtype, device=Wp.device)
-            uniq = ctypes.c_int64(0)
-            with torch.cuda.device(Wp.device):
-                nat.call("gsp_coo_to_csr_" + nat.suffix(Wp.dtype), nat.i64(n),
-                         nat.i64(vals.numel()), rows, cols, vals, indptr, indices, data,
-                         ctypes.byref(uniq), nat.stream_ptr(Wp.device))
-            m = int(uniq.value)
-            W = DeviceCSR(indptr, indices[:m].contiguous(), data[:m].contiguous(), (n, n))
+            W = DeviceCSR.from_coo(torch.cat([row_ids(Wp.indptr), row_ids(Wg.indptr)]),
+                                   torch.cat([Wp.indices, Wg.indices]),
+                                   torch.cat([Wp.data, Wg.data.to(Wp.dtype)]), (h * w, h * w))
         else:
             W = aggregate(self.Gp.W.to_scipy(), self.Gg.W.to_scipy())
         super().__init__(W, coords=self.Gg.coords, plotting=self.Gg.plotting,
                          dtype=dt, device=dev)
-
-
-def _csr_rows(M):
-    """Row id of every stored entry of a DeviceCSR (int32)."""
-    torch = nat.require_cuda()
-    counts = (M.indptr[1:] - M.indptr[:-1]).long()
-    return torch.repeat_interleave(torch.arange(M.shape[0], dtype=torch.int32,
-                                                device=M.device), counts)
 
 
 class Sensor(NNGraph):
@@ -748,23 +728,16 @@ class KnnSlabs:
         if self.backend != "device":
             raise ValueError("laplacian_rows_device needs backend='device'")
         dev, dt = self.points.device, _torch_dtype(torch, dtype)
-        m, k, n = int(self.points.shape[0]), self.k, self.n_per
+        n = self.n_per
         # unused rows (kept points farther than `margin` from the slab) get zero-weight lists:
         # an infinite distance gives exp(-inf) = 0 and the zeros are dropped below
         dist = torch.where(self.used[:, None], self.D, torch.full_like(self.D, float("inf")))
-        indptr = torch.empty(m + 1, dtype=torch.int32, device=dev)
-        indices = torch.empty(m * k, dtype=torch.int32, device=dev)
-        data = torch.empty(m * k, dtype=dt, device=dev)
-        with torch.cuda.device(dev):
-            nat.call("gsp_knn_to_csr_" + nat.suffix(dt), nat.i64(m), nat.i32(k), self.NN, dist,
-                     nat.f64(sigma), indptr, indices, data, nat.stream_ptr(dev))
-        W = symmetrize_average_device(DeviceCSR(indptr, indices, data, (m, m)))
-        del indptr, indices, data, dist
-        ptr = W.indptr[self.own_lo:self.own_lo + n + 1].long()
+        W = _knn_gauss_csr(self.NN, dist, sigma, dt).symmetrize("average")
+        del dist
+        ptr = W.indptr[self.own_lo:self.own_lo + n + 1]
         a, b = int(ptr[0].item()), int(ptr[-1].item())
         cols, vals = W.indices[a:b].long(), W.data[a:b]
-        counts = ptr[1:] - ptr[:-1]
-        rows = torch.repeat_interleave(torch.arange(n, device=dev), counts)
+        rows = row_ids(ptr)
         keep = vals != 0
         rows, vals = rows[keep], vals[keep]
         gcol = self.gid[cols[keep]]

@@ -96,7 +96,7 @@ class Graph(FourierMixIn, DifferenceMixIn, ConnectivityMixIn, LayoutMixIn):
         if stats[2]:
             self.logger.warning("Adjacency: there are negative edge weights.")
         if stats[4]:                                     # graph.py:128 eliminate_zeros()
-            W = self._compact(W)
+            W = W.eliminate_zeros()
         self._adjacency = W
         self._n_loops = int(stats[3])
 
@@ -133,29 +133,14 @@ class Graph(FourierMixIn, DifferenceMixIn, ConnectivityMixIn, LayoutMixIn):
         """Graph from COO triplets already in HBM (int32 rows / cols, float values).
 
         What ``sparse.csr_matrix(coo)`` does at graph.py:109 -- sort by (row, col), sum
-        duplicates -- runs on the device (``gsp_coo_to_csr_*``); no host matrix exists.
+        duplicates -- runs on the device (:meth:`DeviceCSR.from_coo`); no host matrix exists.
         """
-        import ctypes
         torch = nat.require_cuda()
-        dev = vals.device
         dt = _torch_dtype(torch, kwargs.get("dtype", vals.dtype if vals.dtype in
                                             (torch.float32, torch.float64) else None))
-        rows = rows.to(dev, torch.int32).contiguous()
-        cols = cols.to(dev, torch.int32).contiguous()
-        vals = vals.to(dev, dt).contiguous()
-        nnz = int(vals.numel())
-        indptr = torch.empty(n_vertices + 1, dtype=torch.int32, device=dev)
-        indices = torch.empty(nnz, dtype=torch.int32, device=dev)
-        data = torch.empty(nnz, dtype=dt, device=dev)
-        uniq = ctypes.c_int64(0)
-        with torch.cuda.device(dev):
-            nat.call("gsp_coo_to_csr_" + nat.suffix(dt), nat.i64(n_vertices), nat.i64(nnz), rows,
-                     cols, vals, indptr, indices, data, ctypes.byref(uniq), nat.stream_ptr(dev))
-        m = int(uniq.value)
-        W = DeviceCSR(indptr, indices[:m].contiguous(), data[:m].contiguous(),
-                      (n_vertices, n_vertices))
+        W = DeviceCSR.from_coo(rows, cols, vals.to(dt), (n_vertices, n_vertices))
         kwargs.setdefault("dtype", dt)
-        kwargs.setdefault("device", dev)
+        kwargs.setdefault("device", vals.device)
         return cls(W, lap_type=lap_type, **kwargs)
 
     # ------------------------------------------------------------------ basics
@@ -191,18 +176,6 @@ class Graph(FourierMixIn, DifferenceMixIn, ConnectivityMixIn, LayoutMixIn):
         self._call("gsp_csr_inspect", nat.i64(W.shape[0]), W.indptr, W.indices, W.data, stats)
         return stats.cpu().numpy()
 
-    def _compact(self, W):
-        torch = nat.require_cuda()
-        n = W.shape[0]
-        indptr = torch.empty(n + 1, dtype=torch.int32, device=self.device)
-        self._call("gsp_csr_compact_count", nat.i64(n), W.indptr, W.data, indptr)
-        nnz = int(indptr[-1].item()) if n else 0
-        indices = torch.empty(nnz, dtype=torch.int32, device=self.device)
-        data = torch.empty(nnz, dtype=self.dtype, device=self.device)
-        self._call("gsp_csr_compact_fill", nat.i64(n), W.indptr, W.indices, W.data, indptr,
-                   indices, data)
-        return DeviceCSR(indptr, indices, data, W.shape)
-
     def has_loops(self):
         return self._n_loops > 0
 
@@ -220,14 +193,7 @@ class Graph(FourierMixIn, DifferenceMixIn, ConnectivityMixIn, LayoutMixIn):
     # ---------------------------------------------------- symmetric part, degree
     def _transpose(self):
         if self._Wt is None:
-            torch = nat.require_cuda()
-            W, n = self._adjacency, self.n_vertices
-            tp = torch.empty(n + 1, dtype=torch.int32, device=self.device)
-            ti = torch.empty(W.nnz, dtype=torch.int32, device=self.device)
-            td = torch.empty(W.nnz, dtype=self.dtype, device=self.device)
-            self._call("gsp_csr_transpose", nat.i64(n), nat.i64(W.nnz), W.indptr, W.indices,
-                       W.data, tp, ti, td)
-            self._Wt = DeviceCSR(tp, ti, td, W.shape)
+            self._Wt = self._adjacency.transpose()
         return self._Wt
 
     def _symmetric_adjacency(self):
@@ -235,17 +201,7 @@ class Graph(FourierMixIn, DifferenceMixIn, ConnectivityMixIn, LayoutMixIn):
         if not self.is_directed():
             return self._adjacency
         if self._Ws is None:
-            torch = nat.require_cuda()
-            W, Wt, n = self._adjacency, self._transpose(), self.n_vertices
-            sp = torch.empty(n + 1, dtype=torch.int32, device=self.device)
-            self._call("gsp_csr_average_count", nat.i64(n), W.indptr, W.indices, W.data,
-                       Wt.indptr, Wt.indices, Wt.data, sp)
-            nnz = int(sp[-1].item()) if n else 0
-            si = torch.empty(nnz, dtype=torch.int32, device=self.device)
-            sd = torch.empty(nnz, dtype=self.dtype, device=self.device)
-            self._call("gsp_csr_average_fill", nat.i64(n), W.indptr, W.indices, W.data,
-                       Wt.indptr, Wt.indices, Wt.data, sp, si, sd)
-            self._Ws = DeviceCSR(sp, si, sd, W.shape)
+            self._Ws = self._adjacency.symmetrize("average", self._transpose())
         return self._Ws
 
     def _degrees(self):
@@ -445,61 +401,10 @@ def ritz_check(alpha, beta, tol, single_precision, polish_done):
     return theta, m, bool(tiny.size or (ref_rule and (tight or polish_done))), ref_rule
 
 
-def symmetrize_average_device(W):
-    """(W + W^T)/2 of a DeviceCSR, on the device (utils.py:247-248)."""
-    torch = nat.require_cuda()
-    n, dev, sfx = W.shape[0], W.device, nat.suffix(W.dtype)
-
-    def call(name, *args):
-        with torch.cuda.device(dev):
-            nat.call(name + "_" + sfx, *args, nat.stream_ptr(dev))
-    tp = torch.empty(n + 1, dtype=torch.int32, device=dev)
-    ti = torch.empty(W.nnz, dtype=torch.int32, device=dev)
-    td = torch.empty(W.nnz, dtype=W.dtype, device=dev)
-    call("gsp_csr_transpose", nat.i64(n), nat.i64(W.nnz), W.indptr, W.indices, W.data, tp, ti, td)
-    sp = torch.empty(n + 1, dtype=torch.int32, device=dev)
-    call("gsp_csr_average_count", nat.i64(n), W.indptr, W.indices, W.data, tp, ti, td, sp)
-    nnz = int(sp[-1].item()) if n else 0
-    si = torch.empty(nnz, dtype=torch.int32, device=dev)
-    sd = torch.empty(nnz, dtype=W.dtype, device=dev)
-    call("gsp_csr_average_fill", nat.i64(n), W.indptr, W.indices, W.data, tp, ti, td, sp, si, sd)
-    return DeviceCSR(sp, si, sd, W.shape)
-
-
-_SYMMETRIZE_MODES = {"maximum": 0, "fill": 1, "tril": 2, "triu": 3}
-
-
 def symmetrize_device(W, method="average"):
-    """utils.symmetrize(W, method) of a square DeviceCSR, on the device (utils.py:244-277).
-
-    'average' is :func:`symmetrize_average_device`; 'maximum', 'fill', 'tril' and 'triu' merge
-    each row of W with the same row of W^T (``gsp_csr_symmetrize_*``), with the reference's
-    arithmetic, so values are bit-equal to SciPy's in float64.  Exact zeros are dropped."""
-    if W.shape[0] != W.shape[1]:
-        raise ValueError("Matrix must be square.")
-    if method == "average":
-        return symmetrize_average_device(W)
-    if method not in _SYMMETRIZE_MODES:
-        raise ValueError("Unknown symmetrization method {}.".format(method))
-    torch = nat.require_cuda()
-    n, dev, sfx = W.shape[0], W.device, nat.suffix(W.dtype)
-    mode = nat.i32(_SYMMETRIZE_MODES[method])
-
-    def call(name, *args):
-        with torch.cuda.device(dev):
-            nat.call(name + "_" + sfx, *args, nat.stream_ptr(dev))
-    tp = torch.empty(n + 1, dtype=torch.int32, device=dev)
-    ti = torch.empty(W.nnz, dtype=torch.int32, device=dev)
-    td = torch.empty(W.nnz, dtype=W.dtype, device=dev)
-    call("gsp_csr_transpose", nat.i64(n), nat.i64(W.nnz), W.indptr, W.indices, W.data, tp, ti, td)
-    sp = torch.empty(n + 1, dtype=torch.int32, device=dev)
-    call("gsp_csr_symmetrize_count", nat.i64(n), mode, W.indptr, W.indices, W.data, tp, ti, td, sp)
-    nnz = int(sp[-1].item()) if n else 0
-    si = torch.empty(nnz, dtype=torch.int32, device=dev)
-    sd = torch.empty(nnz, dtype=W.dtype, device=dev)
-    call("gsp_csr_symmetrize_fill", nat.i64(n), mode, W.indptr, W.indices, W.data, tp, ti, td, sp,
-         si, sd)
-    return DeviceCSR(sp, si, sd, W.shape)
+    """utils.symmetrize(W, method) of a square DeviceCSR, on the device (utils.py:244-277):
+    :meth:`DeviceCSR.symmetrize`."""
+    return W.symmetrize(method)
 
 
 def _torch_dtype(torch, dtype):

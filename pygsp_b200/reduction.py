@@ -23,6 +23,7 @@ from scipy import sparse
 from . import _native as nat
 from . import filters
 from . import utils
+from .graphs.csr import DeviceCSR, row_ids
 
 logger = utils.build_logger(__name__)
 
@@ -43,14 +44,10 @@ def _ctx():
 def _device_matrix(L, device):
     """A host (SciPy / NumPy) or device square matrix as a canonical float64 DeviceCSR without
     stored zeros: an explicit zero is not an edge (it must not join two components)."""
-    from .graphs.csr import DeviceCSR
     torch = nat.require_cuda()
     if isinstance(L, DeviceCSR):
         M = DeviceCSR(L.indptr, L.indices, L.data.to(torch.float64), L.shape)
-        if bool((M.data == 0).any()):
-            keep = M.data != 0
-            M = _coo_to_csr(M.shape[0], _rows_of(M)[keep], M.indices[keep], M.data[keep])
-        return M
+        return M.eliminate_zeros() if bool((M.data == 0).any()) else M
     if hasattr(L, "to_scipy"):
         L = L.to_scipy()
     host = sparse.csr_matrix(L, dtype=np.float64)
@@ -64,55 +61,6 @@ def _device_matrix(L, device):
 
 def _call(name, *args):
     nat.call(name, *args, nat.stream_ptr())
-
-
-def _rows_of(M):
-    torch = nat.require_cuda()
-    counts = (M.indptr[1:] - M.indptr[:-1]).long()
-    return torch.repeat_interleave(torch.arange(M.shape[0], device=M.device), counts)
-
-
-def _coo_to_csr(n, rows, cols, vals):
-    """Canonical CSR (duplicates summed in emission order) of float64 COO triplets."""
-    import ctypes
-    from .graphs.csr import DeviceCSR
-    torch = nat.require_cuda()
-    dev = vals.device
-    nnz = int(vals.numel())
-    if nnz >= 2 ** 31:
-        raise ValueError("The result would have {} entries; at most 2^31 - 1 are "
-                         "supported.".format(nnz))
-    indptr = torch.empty(n + 1, dtype=torch.int32, device=dev)
-    indices = torch.empty(nnz, dtype=torch.int32, device=dev)
-    data = torch.empty(nnz, dtype=torch.float64, device=dev)
-    uniq = ctypes.c_int64(0)
-    _call("gsp_coo_to_csr_f64", nat.i64(n), nat.i64(nnz), rows.to(torch.int32).contiguous(),
-          cols.to(torch.int32).contiguous(), vals.contiguous(), indptr, indices, data,
-          ctypes.byref(uniq))
-    m = int(uniq.value)
-    return DeviceCSR(indptr, indices[:m].contiguous(), data[:m].contiguous(), (n, n))
-
-
-def _induced_coo(M, v):
-    """Entries of M[v, :][:, v] as COO (rows, cols, vals) for device int32 ids v."""
-    torch = nat.require_cuda()
-    n, m, dev = M.shape[0], int(v.numel()), M.device
-    mptr = torch.empty(n + 1, dtype=torch.int32, device=dev)
-    mpos = torch.empty(max(m, 1), dtype=torch.int32, device=dev)
-    s_indptr = torch.empty(m + 1, dtype=torch.int32, device=dev)
-    nnz = torch.zeros(1, dtype=torch.int64, device=dev)
-    _call("gsp_vertex_map", nat.i64(n), nat.i64(m), v, mptr, mpos)
-    if m == 0:
-        e = torch.empty(0, dtype=torch.int32, device=dev)
-        return e, e, torch.empty(0, dtype=torch.float64, device=dev), s_indptr.zero_()
-    _call("gsp_subgraph_count", nat.i64(m), M.indptr, M.indices, v, mptr, None, s_indptr, nnz)
-    nnz = int(nnz.item())
-    cols = torch.empty(nnz, dtype=torch.int32, device=dev)
-    vals = torch.empty(nnz, dtype=torch.float64, device=dev)
-    rows = torch.empty(nnz, dtype=torch.int32, device=dev)
-    _call("gsp_subgraph_fill_f64", nat.i64(m), M.indptr, M.indices, M.data, v, mptr, mpos, None,
-          s_indptr, cols, vals, rows)
-    return rows, cols, vals, s_indptr
 
 
 def _schur(M, ind, small_max=None):
@@ -130,15 +78,15 @@ def _schur(M, ind, small_max=None):
     slot = torch.zeros(n, dtype=torch.int32, device=dev)
     slot[keep.long()] = -1 - torch.arange(m, dtype=torch.int32, device=dev)
     rem = torch.nonzero(slot == 0).flatten().to(torch.int32)
-    r_rows, r_cols, r_vals, _ = _induced_coo(M, keep)
+    R, r_rows = M.induced(keep)        # unsorted triplets: summed with the blocks' by one sort
     nr = int(rem.numel())
     if nr == 0:
-        return _coo_to_csr(m, r_rows, r_cols, r_vals)
+        return DeviceCSR.from_coo(r_rows, R.indices, R.data, (m, m))
 
     # components of the removed vertices, listed component by component
-    s_rows, s_cols, s_vals, s_ptr = _induced_coo(M, rem)
+    S, _ = M.induced(rem, increasing=True)
     labels = torch.empty(nr, dtype=torch.int32, device=dev)
-    _call("gsp_cc_labels_f64", nat.i64(nr), s_ptr, s_cols, s_vals, nat.i32(0), labels, None)
+    _call("gsp_cc_labels_f64", nat.i64(nr), S.indptr, S.indices, S.data, nat.i32(0), labels, None)
     perm = torch.empty(nr, dtype=torch.int32, device=dev)
     cptr = torch.empty(nr + 1, dtype=torch.int32, device=dev)
     ncomp = torch.empty(1, dtype=torch.int64, device=dev)
@@ -153,7 +101,7 @@ def _schur(M, ind, small_max=None):
     comp_of[cvert.long()] = comp_of_pos
 
     # kept neighbours of every component, in increasing kept index
-    rows, cols = _rows_of(M), M.indices.long()
+    rows, cols = row_ids(M.indptr), M.indices.long()
     edge = (comp_of[rows] >= 0) & (slot[cols] < 0)
     keys = torch.unique(comp_of[rows[edge]] * m + (-1 - slot[cols[edge]].long()))
     bcomp, bidx = keys // m, (keys % m).to(torch.int32).contiguous()
@@ -164,7 +112,7 @@ def _schur(M, ind, small_max=None):
     out_off = torch.zeros(nc + 1, dtype=torch.int64, device=dev)
     out_off[1:] = torch.cumsum(out_len, 0)
     total = int(out_off[-1].item())
-    nnz_red = int(r_vals.numel())
+    nnz_red = R.nnz
     if total + nnz_red >= 2 ** 31:
         raise ValueError("The Kron reduction would have {} entries before summation; at most "
                          "2^31 - 1 are supported.".format(total + nnz_red))
@@ -177,7 +125,7 @@ def _schur(M, ind, small_max=None):
     rows_out = torch.empty(total + nnz_red, dtype=torch.int32, device=dev)
     cols_out = torch.empty(total + nnz_red, dtype=torch.int32, device=dev)
     vals_out = torch.empty(total + nnz_red, dtype=torch.float64, device=dev)
-    rows_out[total:], cols_out[total:], vals_out[total:] = r_rows, r_cols, r_vals
+    rows_out[total:], cols_out[total:], vals_out[total:] = r_rows, R.indices, R.data
     status = torch.zeros(1, dtype=torch.int32, device=dev)
     bptr32 = bptr.to(torch.int32).contiguous()
     comps = torch.nonzero(small).flatten().to(torch.int32).contiguous()
@@ -212,13 +160,12 @@ def _schur(M, ind, small_max=None):
         raise ValueError("Kron reduction: a block of the removed vertices is not positive "
                          "definite (the matrix is not a connected Laplacian-like matrix).")
     # components without kept neighbours emitted nothing: their slots are empty (b = 0)
-    out = _coo_to_csr(m, rows_out, cols_out, vals_out)
+    out = DeviceCSR.from_coo(rows_out, cols_out, vals_out, (m, m))
     # Every block is symmetric and M_red is, but the summation of duplicates need not associate
     # (i, j) and (j, i) alike; average with the transpose if any entry differs (the reference
     # symmetrises an almost symmetric result too, reduction.py:361-362).
     if _asymmetry(out):
-        from .graphs.graph import symmetrize_average_device
-        out = symmetrize_average_device(out)
+        out = out.symmetrize("average")
     return out
 
 
@@ -271,7 +218,7 @@ def kron_reduction(G, ind):
         ind = _kept_ids(ind, G.N)
         with torch.cuda.device(G.device):
             L = _schur(_device_matrix(G.L, G.device), ind)
-            rows = _rows_of(L)
+            rows = row_ids(L.indptr)
             off = rows != L.indices.long()
             Gnew = Graph.from_coo(rows[off], L.indices[off], -L.data[off], len(ind),
                                   lap_type=G.lap_type, dtype=G.dtype, device=G.device,
@@ -300,8 +247,7 @@ def _laplacian_inverse(L):
         raise ValueError("The dense factor of this {0} x {0} Laplacian needs about {1:.1f} GB of "
                          "device memory ({2:.1f} GB free).".format(n, 3 * n * n * 8 / 2 ** 30,
                                                                   free / 2 ** 30))
-    A = torch.zeros((n, n), dtype=torch.float64, device=dev)
-    A[_rows_of(L), L.indices.long()] = L.data
+    A = L.to_dense()
     step = max(1, (1 << 26) // max(n, 1))
     for r0 in range(0, n, step):
         r1 = min(n, r0 + step)
@@ -379,7 +325,7 @@ def graph_sparsify(M, epsilon, maxiter=10, seed=None):
 
     with torch.cuda.device(dev):
         Ld = _device_matrix(L, dev)
-        rows, cols = _rows_of(Ld), Ld.indices.long()
+        rows, cols = row_ids(Ld.indptr), Ld.indices.long()
         w = -Ld.data
         # edges: the lower triangle of W with w >= 1e-10 (reduction.py:89-97)
         edge = (rows > cols) & (w >= 1e-10)
@@ -480,10 +426,11 @@ def _kron_regularized(G, ind, reg_eps):
         L = _device_matrix(G.L, G.device)
         n = G.N
         diag = torch.arange(n, dtype=torch.int32, device=G.device)
-        M = _coo_to_csr(n, torch.cat([_rows_of(L).to(torch.int32), diag]),
-                        torch.cat([L.indices, diag]),
-                        torch.cat([L.data, torch.full((n,), float(reg_eps), dtype=torch.float64,
-                                                      device=G.device)]))
+        M = DeviceCSR.from_coo(torch.cat([row_ids(L.indptr).to(torch.int32), diag]),
+                               torch.cat([L.indices, diag]),
+                               torch.cat([L.data, torch.full((n,), float(reg_eps),
+                                                             dtype=torch.float64,
+                                                             device=G.device)]), (n, n))
         return _schur(M, ind).to_scipy().astype(np.float64)
 
 

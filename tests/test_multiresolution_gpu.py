@@ -169,7 +169,9 @@ def test_kron_reduction_matrix_errors(gsp, monkeypatch):
 
 
 def test_explicit_zero_is_not_an_edge(gsp):
-    """A stored zero between two components does not join them: resistances stay those of pinv."""
+    """A stored zero between two components does not join them: resistances stay those of pinv,
+    for the Laplacian given as a SciPy matrix and as a DeviceCSR (zeros removed on the device)."""
+    import torch
     a = sparse.random(30, 30, density=0.2, random_state=4)
     a = a + a.T
     a.setdiag(0)
@@ -182,8 +184,11 @@ def test_explicit_zero_is_not_an_edge(gsp):
     P = np.linalg.pinv(laplacian(W).toarray())
     d = np.diag(P)
     want = d[:, None] + d[None, :] - 2 * P
-    got = gsp.utils.resistance_distance(L)
-    assert np.abs(got - want).max() <= 1e-9 * np.abs(want).max()
+    Ld = gsp.graphs.DeviceCSR.from_scipy(L, torch.float64, torch.device("cuda"))
+    assert int((Ld.data == 0).sum()) == 2
+    for M in (L, Ld):
+        got = gsp.utils.resistance_distance(M)
+        assert np.abs(got - want).max() <= 1e-9 * np.abs(want).max()
 
 
 def test_largest_eigenvector_chfsi_float32(gsp):

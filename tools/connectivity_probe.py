@@ -59,8 +59,7 @@ def directed_variant(gsp, G):
     """W's structure with the weights above the diagonal doubled, built on the device."""
     import torch
     W = G.W
-    rows = torch.repeat_interleave(torch.arange(G.N, device=G.device, dtype=torch.int32),
-                                   torch.diff(W.indptr).long())
+    rows = gsp.graphs.csr.row_ids(W.indptr)
     data = torch.where(W.indices > rows, W.data * 2, W.data)
     return gsp.graphs.Graph(gsp.graphs.DeviceCSR(W.indptr, W.indices, data, W.shape))
 

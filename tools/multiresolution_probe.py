@@ -55,6 +55,7 @@ def main():
     import pygsp_b200 as gsp
     from pygsp_b200 import _native as nat
     from pygsp_b200 import reduction as red
+    from pygsp_b200.graphs.csr import row_ids
     from scipy.sparse import csgraph
 
     G = gsp.graphs.Sensor(args.n, k=args.k, seed=1, order="morton", dtype=np.float64)
@@ -84,7 +85,7 @@ def main():
     Ld = red._device_matrix(G.L, G.device)
 
     def resist():
-        rows, cols = red._rows_of(Ld), Ld.indices.long()
+        rows, cols = row_ids(Ld.indptr), Ld.indices.long()
         e = rows > cols
         er, ec = rows[e].to(torch.int32).contiguous(), cols[e].to(torch.int32).contiguous()
         A, _, _ = red._laplacian_inverse(Ld)
