@@ -60,6 +60,11 @@ class DistPlan(ctypes.Structure):
                 ("perm", ctypes.c_void_p)]
 
 
+# Scratch of the FISTA solvers (csrc/reduce.cuh): [1] the stop criterion (0 = running), [2] the
+# stop iteration, and the history from this offset (GSPB200_FB_HISTORY = GSPB200_TV_HISTORY).
+FISTA_HISTORY = 3080
+
+
 def header_symbols():
     """Every function name include/gspb200.h declares (macro-expanded)."""
     text = open(_HEADER).read()
@@ -151,3 +156,30 @@ def require_cuda():
     if not torch.cuda.is_available():
         raise NativeError("pygsp_b200 needs a CUDA device (H100): there is no CPU fallback")
     return torch
+
+
+def run_fista(enqueue, batch, last_pass, width, device, what):
+    """Run a FISTA solver to its stop and return ``(scal, niter, crit code, batches)``.
+
+    ``enqueue(it0, it1, cap, scal)`` enqueues passes [it0, it1) on a zero-initialised scratch of
+    ``FISTA_HISTORY + width * cap`` doubles (``width`` history entries per pass).  Batches of
+    ``batch`` passes alternate with reads of the stop record; the history grows by doubling as the
+    run goes on.  ``last_pass`` (None: unbounded) is the pass by which the solver's own rule has
+    stopped it, else ``NativeError`` names the solver ``what``.
+    """
+    torch = require_cuda()
+    cap = 1024 if last_pass is None else min(last_pass + 1, 1024)
+    scal = torch.zeros(FISTA_HISTORY + width * cap, dtype=torch.float64, device=device)
+    done = batches = 0
+    while True:
+        nxt = done + batch if last_pass is None else min(done + batch, last_pass + 1)
+        if nxt > cap:
+            cap = max(2 * cap, nxt) if last_pass is None else min(max(2 * cap, nxt), last_pass + 1)
+            scal = torch.cat([scal, scal.new_zeros(FISTA_HISTORY + width * cap - scal.numel())])
+        enqueue(done, nxt, cap, scal)
+        done, batches = nxt, batches + 1
+        rec = scal[:3].cpu().numpy()
+        if rec[1] != 0:
+            return scal, int(rec[2]), int(rec[1]), batches
+        if last_pass is not None and done > last_pass:
+            raise NativeError("the %s solver did not stop at maxit" % what)

@@ -9,26 +9,20 @@
 //
 // Blocks are row-major (n, k) in float or double; small matrices are double, row-major.
 // Products accumulate in double, also for float blocks.  Every reduction over rows is
-// two-level and ORDER-FIXED: CTA p reduces rows [p*chunk, (p+1)*chunk) in row order into a
-// partial, a second pass adds the partials in p order.  The partition depends only on the
-// shapes, never on the device, so results are bit-reproducible.
+// two-level and ORDER-FIXED (csrc/reduce.cuh): CTA p reduces rows [p*chunk, (p+1)*chunk) in row
+// order into a partial, sum_parts adds the partials in p order.  The partition depends only on
+// the shapes, never on the device, so results are bit-reproducible.
 //
 // The products are register-tiled: a CTA of 16 x 16 threads owns a (16 MT) x (16 MT) output
 // tile, thread (ty, tx) the MT x MT entries (ty + 16 p, tx + 16 q) -- strided, so a warp's
 // shared-memory reads are one broadcast and one 128-byte line.  Slabs of KS rows (Gram) or KS
 // inner indices (combine) are staged in shared memory as double.
-#include "common.cuh"
-#include "gspb200.h"
+#include "reduce.cuh"
 
 namespace gsp {
 namespace {
 
-constexpr int kBlockThreads = 256;
-// Row partitions of a reduction: at most this many partials per output entry for the widest
-// micro tile (two CTAs per SM of an H100 when the output is one tile), 2x / 4x as many for the
-// narrower ones, whose CTAs do less work and whose partials are smaller.  Constants, so that the
-// summation order -- and hence the result -- is the same on every device.
-constexpr int64_t kMaxParts = 264;
+constexpr int kBlockThreads = 256;                  // 16 x 16 threads of a tiled product
 
 template <int MT> struct Tile {
   static constexpr int T = 16 * MT;                 // output tile edge
@@ -95,26 +89,6 @@ block_gram_kernel(int64_t n, const T* __restrict__ A, int64_t ka, const T* __res
   }
 }
 
-// out[e] = sum_{p < parts} part[p][e], p in order
-__global__ void reduce_parts_kernel(int64_t count, int64_t parts, const double* __restrict__ part,
-                                    double* __restrict__ out) {
-  for (int64_t e = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; e < count;
-       e += int64_t(gridDim.x) * blockDim.x) {
-    // loads issued eight at a time, added in p order
-    double s = 0.0;
-    int64_t p = 0;
-    for (; p + 8 <= parts; p += 8) {
-      double v[8];
-#pragma unroll
-      for (int q = 0; q < 8; ++q) v[q] = part[(p + q) * count + e];
-#pragma unroll
-      for (int q = 0; q < 8; ++q) s += v[q];
-    }
-    for (; p < parts; ++p) s += part[p * count + e];
-    out[e] = s;
-  }
-}
-
 // Y[r, j] = sum_i A[r, i] Q[i, j]
 template <typename T, int MT>
 __global__ void __launch_bounds__(kBlockThreads)
@@ -167,13 +141,13 @@ block_combine_kernel(int64_t n, const T* __restrict__ A, int64_t ka, const doubl
 
 // part[p][j] = sum over rows r of part p of (LX[r, j] - theta[j] X[r, j])^2.
 // Lane = column (32 per CTA column group), warp w takes rows w, w + 8, ...; the 8 warp sums
-// are added in warp order.
+// are added in warp order (the order of column_part, csrc/reduce.cuh).
 template <typename T>
-__global__ void __launch_bounds__(kBlockThreads)
+__global__ void __launch_bounds__(kThreads)
 block_residual_kernel(int64_t n, const T* __restrict__ X, const T* __restrict__ LX,
                       const double* __restrict__ theta, int64_t k, int64_t chunk,
                       double* __restrict__ part) {
-  constexpr int W = kBlockThreads / 32;
+  constexpr int W = kWarps;
   __shared__ double sums[W][32];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int64_t j = int64_t(blockIdx.y) * 32 + lane;
@@ -211,23 +185,14 @@ __global__ void block_random_kernel(int64_t count, uint64_t seed, T* __restrict_
     X[i] = T(hash_uniform(seed, (uint64_t)i));
 }
 
-inline int grid_for(int64_t count) {
-  return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(count, kBlockThreads), 4096));
-}
-
-// Adds `parts` partials of `count` doubles into out (or copies the only one).
-int finish_parts(const double* part, int64_t parts, int64_t count, double* out, cudaStream_t st) {
-  reduce_parts_kernel<<<grid_for(count), kBlockThreads, 0, st>>>(count, parts, part, out);
-  GSP_LAUNCH_CHECK("block_reduce_parts");
-  return GSP_OK;
-}
-
 template <typename T, int MT>
 int gram_mt(int64_t n, const T* A, int64_t ka, const T* B, int64_t kb, double* C, cudaStream_t st) {
   constexpr int TT = Tile<MT>::T, KS = Tile<MT>::KS;
   const int64_t ta = ceil_div(ka, TT), tb = ceil_div(kb, TT);
   GSP_REQUIRE(ta < 65536 && tb < 65536, "block too wide");
-  // enough partitions to fill the GPU when the output is a few tiles; one when it is large
+  // enough partitions to fill the GPU when the output is a few tiles, one when it is large: at
+  // most kMaxParts for the widest micro tile, 2x / 4x as many for the narrower ones, whose CTAs
+  // do less work and whose partials are smaller
   const int64_t parts = std::max<int64_t>(
       1, std::min<int64_t>(ceil_div(n, 8 * KS),
                            kMaxParts * (8 / MT) / std::min(ta * tb, kMaxParts * (8 / MT))));
@@ -239,7 +204,7 @@ int gram_mt(int64_t n, const T* A, int64_t ka, const T* B, int64_t kb, double* C
   dim3 grid((unsigned)used, (unsigned)ta, (unsigned)tb);
   block_gram_kernel<T, MT><<<grid, kBlockThreads, 0, st>>>(n, A, ka, B, kb, chunk, part);
   GSP_LAUNCH_CHECK("block_gram");
-  return used > 1 ? finish_parts(part, used, ka * kb, C, st) : GSP_OK;
+  return used > 1 ? sum_parts(part, used, ka * kb, C, st) : GSP_OK;
 }
 
 template <typename T>
@@ -291,28 +256,52 @@ int block_residual(int64_t n, const T* X, const T* LX, const double* theta, int6
   }
   const int64_t cg = ceil_div(k, 32);
   GSP_REQUIRE(cg < 65536, "block too wide");
-  const int64_t parts = std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 1024), kMaxParts));
-  const int64_t chunk = ceil_div(n, parts);
-  const int64_t used = ceil_div(n, chunk);
+  const Parts P = row_parts(n);
   Scratch<double> parts_buf(st);
-  if (used > 1) GSP_CUDA(parts_buf.alloc(used * k));
-  double* part = used > 1 ? parts_buf.get() : out;
-  block_residual_kernel<T><<<dim3((unsigned)used, (unsigned)cg), kBlockThreads, 0, st>>>(
-      n, X, LX, theta, k, chunk, part);
+  if (P.used > 1) GSP_CUDA(parts_buf.alloc(P.used * k));
+  double* part = P.used > 1 ? parts_buf.get() : out;
+  block_residual_kernel<T><<<dim3((unsigned)P.used, (unsigned)cg), kThreads, 0, st>>>(
+      n, X, LX, theta, k, P.chunk, part);
   GSP_LAUNCH_CHECK("block_residual");
-  return used > 1 ? finish_parts(part, used, k, out, st) : GSP_OK;
+  return P.used > 1 ? sum_parts(part, P.used, k, out, st) : GSP_OK;
 }
 
 template <typename T>
 int block_random(int64_t n, int64_t k, uint64_t seed, T* X, cudaStream_t st) {
   GSP_REQUIRE(n >= 0 && k >= 1, "bad sizes");
   if (n == 0) return GSP_OK;
-  block_random_kernel<T><<<grid_for(n * k), kBlockThreads, 0, st>>>(n * k, seed, X);
+  block_random_kernel<T><<<grid_for(n * k), kThreads, 0, st>>>(n * k, seed, X);
   GSP_LAUNCH_CHECK("block_random");
   return GSP_OK;
 }
 
 }  // namespace
+
+__global__ void sum_parts_kernel(int64_t count, int64_t parts, const double* __restrict__ part,
+                                 double* __restrict__ out) {
+  for (int64_t e = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; e < count;
+       e += int64_t(gridDim.x) * blockDim.x) {
+    // loads issued eight at a time, added in p order
+    double s = 0.0;
+    int64_t p = 0;
+    for (; p + 8 <= parts; p += 8) {
+      double v[8];
+#pragma unroll
+      for (int q = 0; q < 8; ++q) v[q] = part[(p + q) * count + e];
+#pragma unroll
+      for (int q = 0; q < 8; ++q) s += v[q];
+    }
+    for (; p < parts; ++p) s += part[p * count + e];
+    out[e] = s;
+  }
+}
+
+int sum_parts(const double* part, int64_t parts, int64_t count, double* out, cudaStream_t st) {
+  sum_parts_kernel<<<grid_for(count), kThreads, 0, st>>>(count, parts, part, out);
+  GSP_LAUNCH_CHECK("sum_parts");
+  return GSP_OK;
+}
+
 }  // namespace gsp
 
 // ------------------------------- C ABI ------------------------------------

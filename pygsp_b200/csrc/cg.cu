@@ -6,34 +6,20 @@
 // (:350-365, as CG on L restricted to the unlabelled vertices).  All columns advance
 // together: the product with L is the SpMM step kernel of the filter path, the vector
 // updates are fused with their dot products, every per-column scalar stays on the device,
-// and reductions are two-level in a fixed order (bit-reproducible, as in csrc/lanczos.cu).
+// and reductions are two-level in a fixed order (bit-reproducible): per-CTA partials, added over
+// the CTAs in order by sum_parts (csrc/reduce.cuh) or by load_totals.
 //
 //   spmm      Q = tau L P                                   (cheby_step, FIRST form, no r)
 //   apply     Q = a.Q + d.P ; partial sums of P.Q per column
 //   update    alpha = rr/pq ; X += alpha P ; R -= alpha Q ; partial sums of R.R
 //   direction beta = rr'/rr ; P = R + beta P ; rr history[it+1] = rr'
+#include "reduce.cuh"
 #include "step.cuh"
 
 namespace gsp {
 
 constexpr int kCgThreads = 256;
 constexpr int kCgMaxBlocks = 1024;
-
-struct CgShape {
-  int cw;        // columns per block pass (power of two >= nsig, <= 256)
-  int rpb;       // rows per block pass
-  int blocks;
-};
-
-static inline CgShape cg_shape(int64_t n, int nsig) {
-  CgShape s;
-  s.cw = 1;
-  while (s.cw < nsig) s.cw *= 2;
-  s.rpb = kCgThreads / s.cw;
-  s.blocks = (int)std::max<int64_t>(
-      1, std::min<int64_t>(ceil_div(n, s.rpb), std::min<int64_t>(int64_t(sm_count()) * 4, kCgMaxBlocks)));
-  return s;
-}
 
 // per-column sum over the block of `v` (threads with the same column c = t % cw), result to
 // out[c]; fixed order.
@@ -75,14 +61,6 @@ cg_init_kernel(int64_t n, int nsig, int cw, const T* __restrict__ B, T* __restri
       acc += double(b) * double(b);
     }
   block_colsum(acc, cw, nsig, part_rr + int64_t(blockIdx.x) * nsig);
-}
-
-__global__ void cg_total_kernel(const double* part, int parts, int nsig, double* out) {
-  for (int c = threadIdx.x; c < nsig; c += blockDim.x) {
-    double acc = 0;
-    for (int b = 0; b < parts; ++b) acc += part[int64_t(b) * nsig + c];
-    out[c] = acc;
-  }
 }
 
 template <typename T>
@@ -153,15 +131,17 @@ int cg_run(int64_t n, int64_t nnz, const int32_t* indptr, const int32_t* indices
            int it0, int it1, int cap, double* scal, cudaStream_t st) {
   GSP_REQUIRE(n >= 1 && nsig >= 1 && nsig <= kCgThreads, "block CG: 1..256 right-hand sides per call");
   GSP_REQUIRE(it0 >= 0 && it0 <= it1 && it1 <= cap, "bad iteration range");
-  const CgShape s = cg_shape(n, nsig);
+  int cw = 1;                                      // columns per block pass: a power of two >= nsig
+  while (cw < nsig) cw *= 2;
+  const int blocks = pass_blocks(n, kCgThreads / cw, kCgMaxBlocks);
   double* rr = scal;
   double* part_pq = scal + int64_t(cap + 1) * nsig;
   double* part_rr = part_pq + int64_t(kCgMaxBlocks) * nsig;
   if (it0 == 0) {
-    cg_init_kernel<T><<<s.blocks, kCgThreads, 0, st>>>(n, nsig, s.cw, B, X, R, P, part_rr);
-    cg_total_kernel<<<1, 256, 0, st>>>(part_rr, s.blocks, nsig, rr);
-    note_launch(1);
+    cg_init_kernel<T><<<blocks, kCgThreads, 0, st>>>(n, nsig, cw, B, X, R, P, part_rr);
     GSP_LAUNCH_CHECK("cg_init");
+    const int rc = sum_parts(part_rr, blocks, nsig, rr, st);
+    if (rc != GSP_OK) return rc;
   }
   Step<T> spmm{nnz, indptr, indices, data};       // Q = tau L P: the first form, no r_i
   spmm.x_cur = P;
@@ -173,13 +153,13 @@ int cg_run(int64_t n, int64_t nnz, const int32_t* indptr, const int32_t* indices
   for (int it = it0; it < it1; ++it) {
     int rc = run_step<T>(spmm, 0, n, nullptr, nullptr, st);
     if (rc != GSP_OK) return rc;
-    cg_apply_kernel<T><<<s.blocks, kCgThreads, 0, st>>>(n, nsig, s.cw, a_row, d_row, P, Q, part_pq);
-    cg_update_kernel<T><<<s.blocks, kCgThreads, 0, st>>>(n, nsig, s.cw, X, R, P, Q,
-                                                         rr + int64_t(it) * nsig, part_pq, s.blocks,
-                                                         part_rr);
-    cg_direction_kernel<T><<<s.blocks, kCgThreads, 0, st>>>(n, nsig, s.cw, R, P,
-                                                            rr + int64_t(it) * nsig, part_rr,
-                                                            s.blocks, rr + int64_t(it + 1) * nsig);
+    cg_apply_kernel<T><<<blocks, kCgThreads, 0, st>>>(n, nsig, cw, a_row, d_row, P, Q, part_pq);
+    cg_update_kernel<T><<<blocks, kCgThreads, 0, st>>>(n, nsig, cw, X, R, P, Q,
+                                                       rr + int64_t(it) * nsig, part_pq, blocks,
+                                                       part_rr);
+    cg_direction_kernel<T><<<blocks, kCgThreads, 0, st>>>(n, nsig, cw, R, P,
+                                                          rr + int64_t(it) * nsig, part_rr,
+                                                          blocks, rr + int64_t(it + 1) * nsig);
     note_launch(2);
     GSP_LAUNCH_CHECK("cg_iteration");
   }

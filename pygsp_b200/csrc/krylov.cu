@@ -9,15 +9,12 @@
 // row-major block V[k], so the SpMM (csrc/cheby.cu) takes a slice of it directly.  Slot k + 1
 // is the residual r of step k until it is normalised into q_{k+1}.
 //
-// Columns never mix.  Every reduction over rows is two-level and ORDER-FIXED, in double also
-// for float blocks: CTA p sums rows [p*chunk, (p+1)*chunk) -- lane = column, warp w takes rows
-// w, w + 8, ... in order, the 8 warp sums are added in warp order -- and a second pass adds the
-// partials in p order.  The partition depends on n only, so a column's bits do not depend on
-// nsig, on the other columns, or on how the columns are chunked.
+// Columns never mix.  Every reduction over rows is the two-level column reduction of
+// csrc/reduce.cuh, in double also for float blocks, so a column's bits do not depend on nsig, on
+// the other columns, or on how the columns are chunked.
 #include <cfloat>
 
-#include "common.cuh"
-#include "gspb200.h"
+#include "reduce.cuh"
 
 namespace gsp {
 namespace {
@@ -32,9 +29,6 @@ inline int spmm(int64_t n, const int32_t* indptr, const int32_t* indices, const 
   return gsp_spmm_f64(n, indptr, indices, data, x, ns, y, st);
 }
 
-constexpr int kThreads = 256;
-constexpr int kWarps = kThreads / 32;
-constexpr int64_t kMaxParts = 264;     // row partitions of a reduction (two CTAs per H100 SM)
 constexpr int kGramTile = 8;           // basis vectors per CTA of the per-column Gram
 constexpr int kFilterTile = 16;        // filters per pass of the combine over V
 constexpr double kBreakdown = 16.0;    // breakdown threshold, in units of the dtype's epsilon
@@ -43,36 +37,11 @@ template <typename T> struct Eps;
 template <> struct Eps<float> { static constexpr double value = FLT_EPSILON; };
 template <> struct Eps<double> { static constexpr double value = DBL_EPSILON; };
 
-struct Parts {
-  int64_t used, chunk;
-};
-
-// the row partition of every reduction: a function of n alone
-inline Parts row_parts(int64_t n) {
-  const int64_t parts = std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 1024), kMaxParts));
-  const int64_t chunk = ceil_div(n, parts);
-  return {ceil_div(n, chunk), chunk};
-}
-
-// the CTA's sum of one double per (warp, lane), warps in order; warp 0 writes it
-__device__ __forceinline__ void store_part(double acc, double (*sums)[32], bool valid,
-                                           double* out) {
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  sums[w][lane] = acc;
-  __syncthreads();
-  if (w == 0 && valid) {
-    double s = 0.0;
-    for (int q = 0; q < kWarps; ++q) s += sums[q][lane];
-    *out = s;
-  }
-}
-
 // part[p][j] = sum over rows of part p of x[r, j]^2
 template <typename T>
 __global__ void __launch_bounds__(kThreads)
 krylov_sumsq_kernel(int64_t n, const T* __restrict__ x, int64_t ns, int64_t chunk,
                     double* __restrict__ part) {
-  __shared__ double sums[kWarps][32];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int64_t j = int64_t(blockIdx.y) * 32 + lane;
   const int64_t rb = int64_t(blockIdx.x) * chunk, re = min(n, rb + chunk);
@@ -82,7 +51,7 @@ krylov_sumsq_kernel(int64_t n, const T* __restrict__ x, int64_t ns, int64_t chun
       const double v = double(x[r * ns + j]);
       acc = fma(v, v, acc);
     }
-  store_part(acc, sums, j < ns, part + int64_t(blockIdx.x) * ns + j);
+  column_part(acc, j < ns, part + int64_t(blockIdx.x) * ns + j);
 }
 
 // r -= beta[j] q_prev[:, j] (no q_prev at step 0); part[p][j] = partial q_k[:, j]^T r[:, j]
@@ -91,7 +60,6 @@ __global__ void __launch_bounds__(kThreads)
 krylov_three_term_kernel(int64_t n, T* __restrict__ r, const T* __restrict__ q,
                          const T* __restrict__ q_prev, const double* __restrict__ beta,
                          int64_t ns, int64_t chunk, double* __restrict__ part) {
-  __shared__ double sums[kWarps][32];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int64_t j = int64_t(blockIdx.y) * 32 + lane;
   const int64_t rb = int64_t(blockIdx.x) * chunk, re = min(n, rb + chunk);
@@ -108,7 +76,7 @@ krylov_three_term_kernel(int64_t n, T* __restrict__ r, const T* __restrict__ q,
       acc = fma(double(q[e]), double(rv), acc);
     }
   }
-  store_part(acc, sums, j < ns, part + int64_t(blockIdx.x) * ns + j);
+  column_part(acc, j < ns, part + int64_t(blockIdx.x) * ns + j);
 }
 
 // r -= alpha[j] q_k[:, j]; with `norm`, part[p][j] = partial ||r[:, j]||^2
@@ -117,7 +85,6 @@ __global__ void __launch_bounds__(kThreads)
 krylov_axpy_kernel(int64_t n, T* __restrict__ r, const T* __restrict__ q,
                    const double* __restrict__ alpha, int64_t ns, int64_t chunk, bool norm,
                    double* __restrict__ part) {
-  __shared__ double sums[kWarps][32];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int64_t j = int64_t(blockIdx.y) * 32 + lane;
   const int64_t rb = int64_t(blockIdx.x) * chunk, re = min(n, rb + chunk);
@@ -131,7 +98,7 @@ krylov_axpy_kernel(int64_t n, T* __restrict__ r, const T* __restrict__ q,
       acc = fma(double(rv), double(rv), acc);
     }
   }
-  if (norm) store_part(acc, sums, j < ns, part + int64_t(blockIdx.x) * ns + j);
+  if (norm) column_part(acc, j < ns, part + int64_t(blockIdx.x) * ns + j);
 }
 
 // Per-column Gram: part[p][i][j] = partial sum_r V[i, r, j] b[r, j] for i < kb.  CTA z takes the
@@ -179,7 +146,6 @@ __global__ void __launch_bounds__(kThreads)
 krylov_cgs_update_kernel(int64_t n, const T* __restrict__ V, int64_t kb,
                          const double* __restrict__ h, T* __restrict__ r, int64_t ns,
                          int64_t chunk, double* __restrict__ part) {
-  __shared__ double sums[kWarps][32];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int64_t j = int64_t(blockIdx.y) * 32 + lane;
   const int64_t rb = int64_t(blockIdx.x) * chunk, re = min(n, rb + chunk);
@@ -194,18 +160,7 @@ krylov_cgs_update_kernel(int64_t n, const T* __restrict__ V, int64_t kb,
       r[e] = rv;
       acc = fma(double(rv), double(rv), acc);
     }
-  store_part(acc, sums, j < ns, part + int64_t(blockIdx.x) * ns + j);
-}
-
-// out[e] = sum_{p < parts} part[p][e], p in order
-__global__ void krylov_reduce_kernel(int64_t count, int64_t parts, const double* __restrict__ part,
-                                     double* __restrict__ out) {
-  for (int64_t e = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; e < count;
-       e += int64_t(gridDim.x) * blockDim.x) {
-    double s = 0.0;
-    for (int64_t p = 0; p < parts; ++p) s += part[p * count + e];
-    out[e] = s;
-  }
+  column_part(acc, j < ns, part + int64_t(blockIdx.x) * ns + j);
 }
 
 // max_r sum_e |A[r, e]|: the infinity norm, a bound of the spectral radius of a symmetric A.
@@ -294,16 +249,6 @@ krylov_combine_kernel(int64_t n, const T* __restrict__ V, int64_t kb, const doub
     if (f0 + t < nf) Y[((f0 + t) * n + row) * ldy + j] = T(acc[t]);
 }
 
-inline int grid_for(int64_t count) {
-  return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(count, kThreads), 4096));
-}
-
-int reduce(const double* part, int64_t parts, int64_t count, double* out, cudaStream_t st) {
-  krylov_reduce_kernel<<<grid_for(count), kThreads, 0, st>>>(count, parts, part, out);
-  GSP_LAUNCH_CHECK("krylov_reduce");
-  return GSP_OK;
-}
-
 template <typename T>
 int krylov_basis(int64_t n, int64_t ncols, const int32_t* indptr, const int32_t* indices,
                  const T* data, const T* x, int64_t ns, int order, T* V, double* alpha,
@@ -330,7 +275,7 @@ int krylov_basis(int64_t n, int64_t ncols, const int32_t* indptr, const int32_t*
   GSP_LAUNCH_CHECK("krylov_norm_bound");
   krylov_sumsq_kernel<T><<<red, kThreads, 0, st>>>(n, x, ns, P.chunk, part);
   GSP_LAUNCH_CHECK("krylov_sumsq");
-  int rc = reduce(part, P.used, ns, ss, st);
+  int rc = sum_parts(part, P.used, ns, ss, st);
   if (rc != GSP_OK) return rc;
   krylov_start_kernel<<<grid_for(ns), kThreads, 0, st>>>(ns, ss, beta, m, den, scale);
   GSP_LAUNCH_CHECK("krylov_start");
@@ -343,7 +288,7 @@ int krylov_basis(int64_t n, int64_t ncols, const int32_t* indptr, const int32_t*
     krylov_three_term_kernel<T><<<red, kThreads, 0, st>>>(
         n, r, q, k ? q - plane : nullptr, beta + int64_t(k) * ns, ns, P.chunk, part);
     GSP_LAUNCH_CHECK("krylov_three_term");
-    if ((rc = reduce(part, P.used, ns, alpha + int64_t(k) * ns, st)) != GSP_OK) return rc;
+    if ((rc = sum_parts(part, P.used, ns, alpha + int64_t(k) * ns, st)) != GSP_OK) return rc;
     if (k == order - 1) break;             // beta_order and q_order are not part of the result
     krylov_axpy_kernel<T><<<red, kThreads, 0, st>>>(n, r, q, alpha + int64_t(k) * ns, ns,
                                                     P.chunk, k == 0, part);
@@ -354,11 +299,11 @@ int krylov_basis(int64_t n, int64_t ncols, const int32_t* indptr, const int32_t*
                                        (unsigned)ceil_div(kb, kGramTile)),
                                   kThreads, 0, st>>>(n, V, kb, r, ns, P.chunk, part);
       GSP_LAUNCH_CHECK("krylov_cgs_gram");
-      if ((rc = reduce(part, P.used, kb * ns, h, st)) != GSP_OK) return rc;
+      if ((rc = sum_parts(part, P.used, kb * ns, h, st)) != GSP_OK) return rc;
       krylov_cgs_update_kernel<T><<<red, kThreads, 0, st>>>(n, V, kb, h, r, ns, P.chunk, part);
       GSP_LAUNCH_CHECK("krylov_cgs_update");
     }
-    if ((rc = reduce(part, P.used, ns, ss, st)) != GSP_OK) return rc;
+    if ((rc = sum_parts(part, P.used, ns, ss, st)) != GSP_OK) return rc;
     krylov_step_kernel<<<grid_for(ns), kThreads, 0, st>>>(
         ns, k, tol, anorm, alpha + int64_t(k) * ns, ss, beta + int64_t(k + 1) * ns, m, den, scale);
     GSP_LAUNCH_CHECK("krylov_step");
@@ -370,7 +315,7 @@ int krylov_basis(int64_t n, int64_t ncols, const int32_t* indptr, const int32_t*
                                    (unsigned)ceil_div(order, kGramTile)),
                               kThreads, 0, st>>>(n, V, order, x, ns, P.chunk, part);
   GSP_LAUNCH_CHECK("krylov_cgs_gram");
-  return reduce(part, P.used, int64_t(order) * ns, vs, st);
+  return sum_parts(part, P.used, int64_t(order) * ns, vs, st);
 }
 
 template <typename T>

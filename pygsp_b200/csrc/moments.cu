@@ -15,11 +15,9 @@
 // Moments.  With T_j T_k = (T_{j+k} + T_{|j-k|}) / 2 and L symmetric,
 //   mu_{2k} = 2 ||T_k e_i||^2 - 1,  mu_{2k+1} = 2 <T_{k+1} e_i, T_k e_i> - mu_1,  mu_1 = <T_1 e_i, e_i>.
 // After step k (T_{k+1} from T_k) one pass sums ||T_{k+1}[:, j]||^2 and <T_{k+1}[:, j], T_k[:, j]>
-// per column, in double also for float blocks, in a fixed order (the scheme of csrc/krylov.cu):
-// CTA p sums rows [p*chunk, (p+1)*chunk) -- lane = column, warp w takes rows w, w + 8, ... in
-// order, the 8 warp sums are added in warp order -- and a second pass adds the partials in p
-// order.  The partition depends on n only, so a vertex's moments do not depend on the block
-// width, its position in the block or the other vertices of the block.
+// per column, in double also for float blocks, by the two-level column reduction of
+// csrc/reduce.cuh, so a vertex's moments do not depend on the block width, its position in the
+// block or the other vertices of the block.
 //
 // Two-hop counts.  For every row i, the number of distinct c with W[i, k] > 0 and W[k, c] > 0
 // for some k (the entries of row i of the boolean product A A) and the number of k with
@@ -31,35 +29,16 @@
 // insertions gives the same integer whatever the insertion order.
 #include <vector>
 
-#include "common.cuh"
-#include "gspb200.h"
+#include "reduce.cuh"
 
 namespace gsp {
 namespace {
 
-constexpr int kThreads = 256;
-constexpr int kWarps = kThreads / 32;
-constexpr int64_t kMaxParts = 264;            // row partitions of a reduction (two CTAs per SM)
 constexpr int kLightCap = 1024;               // candidates of a row counted in shared memory
 constexpr int kLightSlots = 2 * kLightCap;    // hash slots per warp
 constexpr int kLightWarps = 4;                // warps per CTA of the light-row kernel (32 KB)
 constexpr int64_t kHeavySlots = int64_t(1) << 24;   // global hash slots per heavy chunk (64 MB)
 constexpr int kHeavySlices = 32;              // CTAs per heavy row
-
-struct Parts {
-  int64_t used, chunk;
-};
-
-// the row partition of every reduction: a function of n alone (as csrc/krylov.cu)
-inline Parts row_parts(int64_t n) {
-  const int64_t parts = std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 1024), kMaxParts));
-  const int64_t chunk = ceil_div(n, parts);
-  return {ceil_div(n, chunk), chunk};
-}
-
-inline int grid_for(int64_t count) {
-  return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(count, kThreads), 4096));
-}
 
 // X[r, j] = (r == v0 + j): columns v0 .. v0 + b - 1 of the identity, row-major (n, b)
 template <typename T>
@@ -72,7 +51,8 @@ __global__ void probe_block_kernel(int64_t n, int64_t v0, int64_t b, T* __restri
   }
 }
 
-// part[p][0][j] = partial sum of tn[r, j]^2, part[p][1][j] = partial sum of tn[r, j] tc[r, j]
+// part[p][0][j] = partial sum of tn[r, j]^2, part[p][1][j] = partial sum of tn[r, j] tc[r, j],
+// each in the order of column_part (csrc/reduce.cuh)
 template <typename T>
 __global__ void __launch_bounds__(kThreads)
 moments_part_kernel(int64_t n, const T* __restrict__ tn, const T* __restrict__ tc, int64_t b,
@@ -102,17 +82,6 @@ moments_part_kernel(int64_t n, const T* __restrict__ tn, const T* __restrict__ t
     double* out = part + int64_t(blockIdx.x) * 2 * b;
     out[j] = s0;
     out[b + j] = s1;
-  }
-}
-
-// out[e] = sum_{p < parts} part[p][e], p in order
-__global__ void moments_reduce_kernel(int64_t count, int64_t parts,
-                                      const double* __restrict__ part, double* __restrict__ out) {
-  for (int64_t e = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; e < count;
-       e += int64_t(gridDim.x) * blockDim.x) {
-    double s = 0.0;
-    for (int64_t p = 0; p < parts; ++p) s += part[p * count + e];
-    out[e] = s;
   }
 }
 
@@ -274,10 +243,7 @@ int moments_step(int64_t n, const T* tn, const T* tc, int64_t b, int m, int k, d
   moments_part_kernel<T><<<dim3((unsigned)P.used, (unsigned)ceil_div(b, 32)), kThreads, 0, st>>>(
       n, tn, tc, b, P.chunk, part.get());
   GSP_LAUNCH_CHECK("moments_part");
-  moments_reduce_kernel<<<grid_for(2 * b), kThreads, 0, st>>>(2 * b, P.used, part.get(),
-                                                               sums + int64_t(k) * 2 * b);
-  GSP_LAUNCH_CHECK("moments_reduce");
-  return GSP_OK;
+  return sum_parts(part.get(), P.used, 2 * b, sums + int64_t(k) * 2 * b, st);
 }
 
 template <typename T>

@@ -17,6 +17,8 @@
 // Once a test has fired every later row launch returns at once, so the buffer of the stopping
 // iterate is never written again: with X2 = [B0 | B1], iterate k lives in B[k % 2].
 // The one-hot Y is never formed: label[row] is the class of a labelled vertex, -1 otherwise.
+// The scratch has the FISTA layout of csrc/reduce.cuh; its history holds the objective of
+// iterate k at k.
 #include <math.h>
 
 #include "reduce.cuh"
@@ -24,13 +26,7 @@
 
 namespace gsp {
 
-constexpr int kFbThreads = 256;
-constexpr int kFbMaxBlocks = 1024;
 constexpr int kFbMaxClasses = 256;
-// scratch: [0] t of FISTA, [1] stop criterion (0 = running), [2] stop iteration,
-// [3] arrival counter (uint64 bits), [8, 8 + 3 kFbMaxBlocks) partials, then the history.
-constexpr int kFbPart = 8;
-static_assert(GSPB200_FB_HISTORY == kFbPart + 3 * kFbMaxBlocks, "scratch layout");
 
 enum { kCritNone = 0, kCritAtol = 1, kCritDtol = 2, kCritRtol = 3, kCritXtol = 4, kCritMaxit = 5 };
 
@@ -40,7 +36,7 @@ struct FbStop {
 };
 
 template <typename T>
-__global__ void __launch_bounds__(kFbThreads)
+__global__ void __launch_bounds__(kThreads)
 fb_init_kernel(int64_t n, int C, const int32_t* __restrict__ label, T* __restrict__ X0,
                double* scal) {
   if (blockIdx.x == 0 && threadIdx.x == 0) {
@@ -61,7 +57,7 @@ fb_init_kernel(int64_t n, int C, const int32_t* __restrict__ label, T* __restric
 // w = 2^ceil(log2 C) lanes per row (32 / w rows per warp); V > 1 a warp per row (w = 32).
 // Xprev may alias Xout (every element is read before the same thread overwrites it).
 template <typename T, int V>
-__global__ void __launch_bounds__(kFbThreads)
+__global__ void __launch_bounds__(kThreads)
 fb_row_kernel(int64_t n, int C, int w, const int32_t* __restrict__ label,
               const T* __restrict__ Xk, const T* Xprev, const T* __restrict__ LXk,
               const T* __restrict__ LXprev, T* Xout, double tau, double step, int it, FbStop stop,
@@ -70,7 +66,7 @@ fb_row_kernel(int64_t n, int C, int w, const int32_t* __restrict__ label,
   const double t = scal[0];
   const double tn = (1.0 + sqrt(1.0 + 4.0 * t * t)) / 2.0;
   const double beta = (t - 1.0) / tn;
-  const int lane = threadIdx.x % w, g = threadIdx.x / w, rpb = kFbThreads / w;
+  const int lane = threadIdx.x % w, g = threadIdx.x / w, rpb = kThreads / w;
   double a_lap = 0, a_fit = 0, a_dx = 0;
   for (int64_t r0 = int64_t(blockIdx.x) * rpb; r0 < n; r0 += int64_t(gridDim.x) * rpb) {
     const int64_t row = r0 + g;                    // r0 is block-uniform: every lane iterates
@@ -128,43 +124,10 @@ fb_row_kernel(int64_t n, int C, int w, const int32_t* __restrict__ label,
     }
   }
 
-  // block partials in a fixed order: warp butterflies, then the warps in order
-  __shared__ double sh[3][kFbThreads / 32];
-  __shared__ bool last;
-  a_lap = group_sum(a_lap, 32);
-  a_fit = group_sum(a_fit, 32);
-  a_dx = group_sum(a_dx, 32);
-  const int warp = threadIdx.x / 32, wl = threadIdx.x % 32;
-  if (wl == 0) { sh[0][warp] = a_lap; sh[1][warp] = a_fit; sh[2][warp] = a_dx; }
-  __syncthreads();
-  double* part = scal + kFbPart;
-  if (threadIdx.x < 3) {
-    double acc = 0;
-    for (int k = 0; k < kFbThreads / 32; ++k) acc += sh[threadIdx.x][k];
-    part[int64_t(blockIdx.x) * 3 + threadIdx.x] = acc;
-    __threadfence();
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    unsigned long long* counter = reinterpret_cast<unsigned long long*>(scal) + 3;
-    last = atomicAdd(counter, 1ull) == (unsigned long long)(gridDim.x - 1);
-  }
-  __syncthreads();
-  if (!last) return;
-
-  // the last block: totals over the blocks (warp q sums quantity q, lanes strided, then a
-  // butterfly -- a fixed order for a given grid), objective, stop tests
-  __threadfence();
-  if (warp < 3) {
-    double acc = 0;
-    for (int b = wl; b < int(gridDim.x); b += 32) acc += __ldcg(part + int64_t(b) * 3 + warp);
-    acc = group_sum(acc, 32);
-    if (wl == 0) sh[warp][0] = acc;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double* obj = scal + GSPB200_FB_HISTORY;
-    const double cur = tau * sh[0][0] + sh[1][0];
+  const double sums[3] = {a_lap, a_fit, a_dx};
+  fista_last_block(sums, scal, [&](const double (&tot)[3]) {   // objective, stop rule
+    double* obj = scal + kFistaHistory;
+    const double cur = tau * tot[0] + tot[1];
     obj[it] = cur;
     int crit = kCritNone;
     if (it >= 1) {
@@ -174,7 +137,7 @@ fb_row_kernel(int64_t n, int C, int w, const int32_t* __restrict__ label,
       double div = cur;
       if (div == 0) div = prev != 0 ? prev : 1.0;
       if (fabs((cur - prev) / div) < stop.rtol) crit = kCritRtol;
-      if (sqrt(sh[2][0]) / sqrt(double(n) * double(C)) < stop.xtol) crit = kCritXtol;
+      if (sqrt(tot[2]) / sqrt(double(n) * double(C)) < stop.xtol) crit = kCritXtol;
       if (stop.maxit >= 0 && it >= stop.maxit) crit = kCritMaxit;
     }
     if (crit != kCritNone) {
@@ -182,18 +145,7 @@ fb_row_kernel(int64_t n, int C, int w, const int32_t* __restrict__ label,
       scal[1] = double(crit);
     }
     scal[0] = tn;
-    reinterpret_cast<unsigned long long*>(scal)[3] = 0ull;
-  }
-}
-
-template <typename T, int V>
-static int launch_row(int blocks, int64_t n, int C, int w, const int32_t* label, const T* Xk,
-                      const T* Xprev, const T* LXk, const T* LXprev, T* Xout, double tau,
-                      double step, int it, const FbStop& stop, double* scal, cudaStream_t st) {
-  fb_row_kernel<T, V><<<blocks, kFbThreads, 0, st>>>(n, C, w, label, Xk, Xprev, LXk, LXprev, Xout,
-                                                     tau, step, it, stop, scal);
-  GSP_LAUNCH_CHECK("fb_row_kernel");
-  return GSP_OK;
+  });
 }
 
 template <typename T>
@@ -208,19 +160,13 @@ int fb_simplex_run(int64_t n, int64_t nnz, const int32_t* indptr, const int32_t*
   GSP_REQUIRE(tau > 0 && step > 0, "tau and step must be positive");
   GSP_REQUIRE(tol != nullptr, "tol_host is required");
   const FbStop stop{tol[0], tol[1], tol[2], tol[3], maxit};
-  int w = 1, V = 1;
-  if (C <= 32) {
-    while (w < C) w *= 2;
-  } else {
-    w = 32;
-    while (32 * V < C) V *= 2;
-  }
-  const int blocks = pass_blocks(n, kFbThreads / w, kFbMaxBlocks);
+  const Lanes lanes = fista_lanes(C);               // V <= 8 for C <= 256: one chunk of columns
+  const int blocks = pass_blocks(n, kThreads / lanes.w, kFistaMaxBlocks);
   const int64_t nc = n * C;
   if (it0 == 0) {
-    const int ib = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(nc, kFbThreads),
+    const int ib = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(nc, kThreads),
                                                                  int64_t(sm_count()) * 8));
-    fb_init_kernel<T><<<ib, kFbThreads, 0, st>>>(n, C, label, X2, scal);
+    fb_init_kernel<T><<<ib, kThreads, 0, st>>>(n, C, label, X2, scal);
     GSP_LAUNCH_CHECK("fb_init_kernel");
   }
   Step<T> lap{nnz, indptr, indices, data};        // L X_k: the first form, alpha = 1, no r_i
@@ -240,12 +186,12 @@ int fb_simplex_run(int64_t n, int64_t nnz, const int32_t* indptr, const int32_t*
     lap.x_new = lap.r = LXk;
     int rc = run_step<T>(lap, 0, n, plan, nullptr, st);
     if (rc != GSP_OK) return rc;
-    switch (V) {
-      case 1: rc = launch_row<T, 1>(blocks, n, C, w, label, Xk, Xp, LXk, LXp, Xo, tau, step, it, stop, scal, st); break;
-      case 2: rc = launch_row<T, 2>(blocks, n, C, w, label, Xk, Xp, LXk, LXp, Xo, tau, step, it, stop, scal, st); break;
-      case 4: rc = launch_row<T, 4>(blocks, n, C, w, label, Xk, Xp, LXk, LXp, Xo, tau, step, it, stop, scal, st); break;
-      default: rc = launch_row<T, 8>(blocks, n, C, w, label, Xk, Xp, LXk, LXp, Xo, tau, step, it, stop, scal, st); break;
-    }
+    rc = launch_lanes(lanes, [&](auto V) {
+      fb_row_kernel<T, decltype(V)::value><<<blocks, kThreads, 0, st>>>(
+          n, C, lanes.w, label, Xk, Xp, LXk, LXp, Xo, tau, step, it, stop, scal);
+      GSP_LAUNCH_CHECK("fb_row_kernel");
+      return GSP_OK;
+    });
     if (rc != GSP_OK) return rc;
   }
   return GSP_OK;

@@ -24,21 +24,14 @@
 //
 // Every element's arithmetic is the same whatever Nsig and the lane packing, so column j of a
 // block follows the single-column iteration bit for bit; only the sums (and so the stop test)
-// see the other columns.
+// see the other columns.  The scratch has the FISTA layout of csrc/reduce.cuh; its history holds
+// P_k and gap_k at 2 k and 2 k + 1.
 #include <math.h>
 
 #include "reduce.cuh"
 #include "step.cuh"
 
 namespace gsp {
-
-constexpr int kTvThreads = 256;
-constexpr int kTvMaxBlocks = 1024;
-// scratch: [0] t_k of FISTA, [1] stop criterion (0 = running), [2] stop iteration,
-// [3] arrival counter (uint64 bits), [8, 8 + 3 kTvMaxBlocks) partials, then the history:
-// P_k and gap_k at 2 k and 2 k + 1.
-constexpr int kTvPart = 8;
-static_assert(GSPB200_TV_HISTORY == kTvPart + 3 * kTvMaxBlocks, "scratch layout");
 
 enum { kTvRunning = 0, kTvRtol = 1, kTvMaxit = 2 };
 
@@ -47,7 +40,7 @@ enum { kTvRunning = 0, kTvRtol = 1, kTvMaxit = 2 };
 // in chunks of 32 V columns.  Uo holds u_{k-1} on entry and u_{k+1} on exit, Gk g_{k-1} and g_k:
 // each element is read before the same thread overwrites it.
 template <typename T, int V>
-__global__ void __launch_bounds__(kTvThreads)
+__global__ void __launch_bounds__(kThreads)
 tv_edge_kernel(int64_t n, int64_t ne, int nsig, int w, const int32_t* __restrict__ dt_indptr,
                const int32_t* __restrict__ dt_indices, const T* __restrict__ dt_data,
                const T* __restrict__ wv, const T* __restrict__ x, const T* __restrict__ z,
@@ -57,7 +50,7 @@ tv_edge_kernel(int64_t n, int64_t ne, int nsig, int w, const int32_t* __restrict
   const double t = it == 0 ? 1.0 : scal[0];
   const double tn = (1.0 + sqrt(1.0 + 4.0 * t * t)) / 2.0;
   const double b = (t - 1.0) / tn;
-  const int lane = threadIdx.x % w, grp = threadIdx.x / w, epb = kTvThreads / w;
+  const int lane = threadIdx.x % w, grp = threadIdx.x / w, epb = kThreads / w;
   double a_l1 = 0, a_gap = 0, a_v = 0;
   for (int64_t e0 = int64_t(blockIdx.x) * epb; e0 < ne; e0 += int64_t(gridDim.x) * epb) {
     const int64_t e = e0 + grp;
@@ -94,51 +87,18 @@ tv_edge_kernel(int64_t n, int64_t ne, int nsig, int w, const int32_t* __restrict
     }
   }
   const int64_t nv = n * nsig;
-  for (int64_t i = int64_t(blockIdx.x) * kTvThreads + threadIdx.x; i < nv;
-       i += int64_t(gridDim.x) * kTvThreads) {
+  for (int64_t i = int64_t(blockIdx.x) * kThreads + threadIdx.x; i < nv;
+       i += int64_t(gridDim.x) * kThreads) {
     const double d = double(__ldg(x + i)) - double(__ldg(z + i));
     a_v += d * d;
   }
 
-  // block partials in a fixed order: warp butterflies, then the warps in order
-  __shared__ double sh[3][kTvThreads / 32];
-  __shared__ bool last;
-  a_l1 = group_sum(a_l1, 32);
-  a_gap = group_sum(a_gap, 32);
-  a_v = group_sum(a_v, 32);
-  const int warp = threadIdx.x / 32, wl = threadIdx.x % 32;
-  if (wl == 0) { sh[0][warp] = a_l1; sh[1][warp] = a_gap; sh[2][warp] = a_v; }
-  __syncthreads();
-  double* part = scal + kTvPart;
-  if (threadIdx.x < 3) {
-    double acc = 0;
-    for (int k = 0; k < kTvThreads / 32; ++k) acc += sh[threadIdx.x][k];
-    part[int64_t(blockIdx.x) * 3 + threadIdx.x] = acc;
-    __threadfence();
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    unsigned long long* counter = reinterpret_cast<unsigned long long*>(scal) + 3;
-    last = atomicAdd(counter, 1ull) == (unsigned long long)(gridDim.x - 1);
-  }
-  __syncthreads();
-  if (!last) return;
-
-  // the last block: totals over the blocks (warp q sums quantity q, lanes strided, then a
-  // butterfly -- a fixed order for a given grid), objective, gap, stop rule
-  __threadfence();
-  if (warp < 3) {
-    double acc = 0;
-    for (int bl = wl; bl < int(gridDim.x); bl += 32) acc += __ldcg(part + int64_t(bl) * 3 + warp);
-    acc = group_sum(acc, 32);
-    if (wl == 0) sh[warp][0] = acc;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double* obj = scal + GSPB200_TV_HISTORY;
-    const double cur = 0.5 * sh[2][0] + gamma * sh[0][0];
+  const double sums[3] = {a_l1, a_gap, a_v};
+  fista_last_block(sums, scal, [&](const double (&tot)[3]) {   // objective, gap, stop rule
+    double* obj = scal + kFistaHistory;
+    const double cur = 0.5 * tot[2] + gamma * tot[0];
     obj[2 * it] = cur;
-    obj[2 * it + 1] = gamma * sh[1][0];
+    obj[2 * it + 1] = gamma * tot[1];
     int crit = kTvRunning;
     if (it >= 1) {
       const double prev = obj[2 * (it - 1)];
@@ -150,8 +110,7 @@ tv_edge_kernel(int64_t n, int64_t ne, int nsig, int w, const int32_t* __restrict
       scal[1] = double(crit);
     }
     scal[0] = tn;
-    reinterpret_cast<unsigned long long*>(scal)[3] = 0ull;
-  }
+  });
 }
 
 // z = x - gamma D u: the step kernel's non-first form on the rectangular D.  That form also reads
@@ -181,34 +140,19 @@ struct TvEdges {
   int maxit, cap;
 };
 
-template <typename T, int V>
-static int launch_edges(const TvEdges& p, int w, const T* dt_data, const T* wv, const T* x,
-                        const T* z, T* U2, T* G, int it, double* scal, cudaStream_t st) {
-  const int64_t blk = p.ur * p.nsig;
-  const int blocks = pass_blocks(std::max(p.ne, p.n), kTvThreads / w, kTvMaxBlocks);
-  tv_edge_kernel<T, V><<<blocks, kTvThreads, 0, st>>>(
-      p.n, p.ne, p.nsig, w, p.dt_indptr, p.dt_indices, dt_data, wv, x, z, U2 + (it % 2) * blk,
-      U2 + ((it + 1) % 2) * blk, G, p.gamma, p.tau, p.tol, it, p.maxit, scal);
-  GSP_LAUNCH_CHECK("tv_edge_kernel");
-  return GSP_OK;
-}
-
 template <typename T>
 int tv_edges(const TvEdges& p, const T* dt_data, const T* wv, const T* x, const T* z, T* U2, T* G,
              int it, double* scal, cudaStream_t st) {
-  int w = 1, V = 1;
-  if (p.nsig <= 32) {
-    while (w < p.nsig) w *= 2;
-  } else {
-    w = 32;
-    while (32 * V < p.nsig && V < 8) V *= 2;
-  }
-  switch (V) {
-    case 1: return launch_edges<T, 1>(p, w, dt_data, wv, x, z, U2, G, it, scal, st);
-    case 2: return launch_edges<T, 2>(p, w, dt_data, wv, x, z, U2, G, it, scal, st);
-    case 4: return launch_edges<T, 4>(p, w, dt_data, wv, x, z, U2, G, it, scal, st);
-    default: return launch_edges<T, 8>(p, w, dt_data, wv, x, z, U2, G, it, scal, st);
-  }
+  const Lanes lanes = fista_lanes(p.nsig);
+  const int64_t blk = p.ur * p.nsig;
+  const int blocks = pass_blocks(std::max(p.ne, p.n), kThreads / lanes.w, kFistaMaxBlocks);
+  return launch_lanes(lanes, [&](auto V) {
+    tv_edge_kernel<T, decltype(V)::value><<<blocks, kThreads, 0, st>>>(
+        p.n, p.ne, p.nsig, lanes.w, p.dt_indptr, p.dt_indices, dt_data, wv, x, z,
+        U2 + (it % 2) * blk, U2 + ((it + 1) % 2) * blk, G, p.gamma, p.tau, p.tol, it, p.maxit, scal);
+    GSP_LAUNCH_CHECK("tv_edge_kernel");
+    return GSP_OK;
+  });
 }
 
 static int tv_check(const TvEdges& p, int it0, int it1) {

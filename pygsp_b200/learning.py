@@ -21,7 +21,6 @@ logger = utils.build_logger(__name__)
 # iterations enqueued between two reads of the simplex solver's stop record
 SIMPLEX_BATCH = 16
 MAX_CLASSES = 256
-_FB_HISTORY = 3080                      # GSPB200_FB_HISTORY (include/gspb200.h)
 _CRITS = {1: "ATOL", 2: "DTOL", 3: "RTOL", 4: "XTOL", 5: "MAXIT"}
 _SOLVE_DEFAULTS = {"atol": None, "dtol": None, "rtol": 1e-3, "xtol": None, "maxit": 200,
                    "verbosity": "LOW"}
@@ -97,34 +96,23 @@ def classification_tikhonov_simplex(G, y, M, tau=0.1, **kwargs):
     maxit = opts["maxit"]
     # iteration k's objective is formed by the k-th row pass: maxit stops by pass max(maxit, 1)
     last_pass = None if maxit is None else max(int(maxit), 1)
-    cap = last_pass + 1 if last_pass is not None else 1024
     tol = np.array([np.nan if opts[k] is None else float(opts[k])
                     for k in ("atol", "dtol", "rtol", "xtol")], dtype=np.float64)
     X2 = torch.empty(2 * n * C, dtype=G.dtype, device=G.device)
     LX2 = torch.empty_like(X2)
     plan = L.tile_plan(C, 0)
+
+    def enqueue(it0, it1, cap, scal):
+        nat.call("gsp_fb_simplex_" + nat.suffix(G.dtype), nat.i64(n), nat.i64(L.nnz), L.indptr,
+                 L.indices, L.data, label, nat.i64(C), nat.f64(tau), nat.f64(step), tol,
+                 nat.i32(-1 if maxit is None else maxit), X2, LX2, nat.i32(it0), nat.i32(it1),
+                 nat.i32(cap), scal, plan, nat.stream_ptr(G.device))
+
     with torch.cuda.device(G.device):
-        scal = torch.zeros(_FB_HISTORY + cap, dtype=torch.float64, device=G.device)
-        done, batches = 0, 0
-        while True:
-            nxt = done + SIMPLEX_BATCH
-            if last_pass is not None:
-                nxt = min(nxt, last_pass + 1)
-            elif nxt > cap:                                  # maxit=None: grow the history
-                cap = max(2 * cap, nxt)
-                scal = torch.cat([scal, scal.new_zeros(_FB_HISTORY + cap - scal.numel())])
-            nat.call("gsp_fb_simplex_" + nat.suffix(G.dtype), nat.i64(n), nat.i64(L.nnz),
-                     L.indptr, L.indices, L.data, label, nat.i64(C), nat.f64(tau), nat.f64(step),
-                     tol, nat.i32(-1 if maxit is None else maxit), X2, LX2, nat.i32(done),
-                     nat.i32(nxt), nat.i32(cap), scal, plan, nat.stream_ptr(G.device))
-            done, batches = nxt, batches + 1
-            rec = scal[:3].cpu().numpy()
-            if rec[1] != 0:
-                break
-            if last_pass is not None and done > last_pass:
-                raise nat.NativeError("the simplex solver did not stop at maxit")
-    niter, crit = int(rec[2]), _CRITS[int(rec[1])]
-    obj = scal[_FB_HISTORY:_FB_HISTORY + niter + 1].cpu().numpy()
+        scal, niter, code, batches = nat.run_fista(enqueue, SIMPLEX_BATCH, last_pass, 1, G.device,
+                                                   "simplex")
+    crit = _CRITS[code]
+    obj = scal[nat.FISTA_HISTORY:nat.FISTA_HISTORY + niter + 1].cpu().numpy()
     last_solve = {"niter": niter, "crit": crit, "objective": obj, "batches": batches}
     if opts["verbosity"] in ("HIGH", "ALL"):
         for k in range(1, niter + 1):

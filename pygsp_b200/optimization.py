@@ -15,7 +15,6 @@ logger = utils.build_logger(__name__)
 
 # iterations enqueued between two reads of the stop record
 TV_BATCH = 16
-_TV_HISTORY = 3080                      # GSPB200_TV_HISTORY (include/gspb200.h)
 _CRITS = {1: "RTOL", 2: "MAXIT"}
 
 # the last prox_tv run: {'niter', 'crit', 'objective', 'gap'}
@@ -124,7 +123,6 @@ def _solve(G, D, X, gamma, A, At, nu, tol, maxit):
     ne = D.shape[1]
     Dt = D.T
     tau = 1.0 / (gamma * 2.0 * G.lmax * nu)
-    cap = min(maxit + 1, 1024)            # history entries; grown as the run goes on
     sfx = nat.suffix(G.dtype)
     stream = nat.stream_ptr(G.device)
     ur = max(n, ne)
@@ -134,7 +132,6 @@ def _solve(G, D, X, gamma, A, At, nu, tol, maxit):
         # rows past Ne stay zero (the vertex pass reads them times 0)
         U2 = torch.zeros(2 * ur * nsig, dtype=G.dtype, device=G.device)
         Gk = torch.zeros(ne * nsig, dtype=G.dtype, device=G.device)
-        scal = torch.zeros(_TV_HISTORY + 2 * cap, dtype=torch.float64, device=G.device)
         blk = ur * nsig
 
         def u_block(k):
@@ -150,33 +147,24 @@ def _solve(G, D, X, gamma, A, At, nu, tol, maxit):
                 V = _apply(At, "At", Du, (n, nsig), G.dtype)
                 torch.add(X, V, alpha=-gamma, out=Z)
 
-        done = 0
-        while True:
-            nxt = min(done + TV_BATCH, maxit + 1)
-            if nxt > cap:
-                cap = min(max(2 * cap, nxt), maxit + 1)
-                scal = torch.cat([scal, scal.new_zeros(_TV_HISTORY + 2 * cap - scal.numel())])
+        def enqueue(it0, it1, cap, scal):
             if A is None:
                 nat.call("gsp_prox_tv_" + sfx, nat.i64(n), nat.i64(ne), nat.i64(D.nnz), D.indptr,
                          D.indices, D.data, Dt.indptr, Dt.indices, Dt.data, X, nat.i64(nsig),
                          nat.f64(gamma), nat.f64(tau), nat.f64(tol), nat.i32(maxit), Z, U2, Gk,
-                         nat.i32(done), nat.i32(nxt), nat.i32(cap), scal, stream)
+                         nat.i32(it0), nat.i32(it1), nat.i32(cap), scal, stream)
             else:
-                for k in range(done, nxt):
+                for k in range(it0, it1):
                     primal(k)
                     W = _apply(A, "A", Z, (n, nsig), G.dtype)
                     nat.call("gsp_prox_tv_edges_" + sfx, nat.i64(n), nat.i64(ne), Dt.indptr,
                              Dt.indices, Dt.data, W, X, Z, nat.i64(nsig), nat.f64(gamma),
                              nat.f64(tau), nat.f64(tol), nat.i32(maxit), U2, Gk, nat.i32(k),
                              nat.i32(cap), scal, stream)
-            done = nxt
-            rec = scal[:3].cpu().numpy()
-            if rec[1] != 0:
-                break
-            if done > maxit:
-                raise nat.NativeError("the TV solver did not stop at maxit")
-        niter, crit = int(rec[2]), _CRITS[int(rec[1])]
+
+        scal, niter, code, _ = nat.run_fista(enqueue, TV_BATCH, maxit, 2, G.device, "TV")
+        crit = _CRITS[code]
         primal(niter)                    # z_niter: later vertex passes overwrote it
-    hist = scal[_TV_HISTORY:_TV_HISTORY + 2 * (niter + 1)].cpu().numpy().reshape(-1, 2)
+    hist = scal[nat.FISTA_HISTORY:nat.FISTA_HISTORY + 2 * (niter + 1)].cpu().numpy().reshape(-1, 2)
     return Z, {"niter": niter, "crit": crit, "objective": hist[:, 0].copy(),
                "gap": hist[:, 1].copy()}

@@ -21,6 +21,16 @@ def test_library_exports_every_declared_symbol():
     assert lib.gsp_abi_version() == 2
 
 
+def test_fista_history_matches_header():
+    """The host reads the FISTA solvers' history at the offset both header macros give."""
+    import re
+    from pygsp_b200 import _native
+    text = open(_native._HEADER).read()
+    for macro in ("GSPB200_FB_HISTORY", "GSPB200_TV_HISTORY"):
+        value = re.search(r"#define %s (\d+)" % macro, text)
+        assert value and int(value.group(1)) == _native.FISTA_HISTORY, macro
+
+
 def test_no_cpu_fallback():
     """Without a CUDA device the product path must fail loudly, not compute on the CPU."""
     import torch

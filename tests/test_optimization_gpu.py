@@ -297,7 +297,7 @@ def test_device_pool_released(gsp, pool_used):
     with pytest.raises(nat.NativeError, match="bad iteration range"):
         import torch
         z = torch.empty(G.N * 3, dtype=torch.float64, device="cuda")
-        scal = torch.zeros(3080 + 2, dtype=torch.float64, device="cuda")
+        scal = torch.zeros(nat.FISTA_HISTORY + 2, dtype=torch.float64, device="cuda")
         D = G.D
         nat.call("gsp_prox_tv_f64", nat.i64(G.N), nat.i64(G.Ne), nat.i64(D.nnz), D.indptr,
                  D.indices, D.data, D.T.indptr, D.T.indices, D.T.data, z, nat.i64(3),

@@ -31,7 +31,7 @@ def category(name):
         return "reorth"
     if "krylov_combine" in name:
         return "combine"
-    if "krylov" in name:
+    if "krylov" in name or "sum_parts" in name:          # sum_parts: the Krylov partials sums
         return "other_lanczos"
     return "other"
 
