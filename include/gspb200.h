@@ -179,6 +179,46 @@ int gsp_cheby_pair_plan_host(int64_t n, const int32_t* indptr_host, const int32_
                              int32_t* nbr_idx, int32_t* slots_fwd, int32_t* slots_rev,
                              int64_t* nbr_count_out);
 int gsp_cheby_clenshaw_pairs_wanted(int64_t n, int64_t nsig, const gsp_tile_plan* plan_host);
+
+/* Neighbour rings of the tiled Clenshaw steps, once per (matrix, rows_per_tile).  The ring of tile
+ * t (rows [t R, t R + R), t < T = n / R) is the sorted union of the tile's own rows and the
+ * columns its rows reference.  A tiled step with a ring copies the tile's ring rows of the
+ * gathered block into shared memory (one 1-D bulk copy per run of consecutive rows) and gathers
+ * from there; the CSR slab then carries 16-bit ring positions instead of column ids.
+ *
+ * gsp_cheby_ring_plan_host: pure host code on HOST copies of indptr / indices.  Writes, per full
+ *   tile, tile_meta[4 t .. 4 t + 4) = {first run, end of runs, ring rows, ring position of row
+ *   t R}; per run, runs[2 i .. 2 i + 2) = {first row, ring position}; per stored entry j of a
+ *   full tile, local[j] = the ring position of indices[j] (0 past the last full tile).
+ *   *ring_max_out receives the rows of the largest ring, *run_count_out the number of runs; when
+ *   that exceeds run_capacity, or the largest ring exceeds 65535 rows, only the two counts are
+ *   written.
+ * gsp_cheby_ring_fits: 1 when a ring of ring_max rows fits the shared memory of a tiled step of
+ *   nsig signals under this tile plan, else 0 (GSPB200_TILE_RING=0 also gives 0: an A/B probe).
+ * gsp_cheby_clenshaw_ring_f32: gsp_cheby_clenshaw_f32 (slots_fwd == NULL) or
+ *   gsp_cheby_clenshaw_pairs_f32 (the pair tables given) with the rings of ring_host, whose
+ *   pointers are device copies of the plan above for plan_host->rows_per_tile; ring_host may be
+ *   NULL (no ring).  Same bits either way. */
+typedef struct gsp_ring_plan {
+  int rows_per_tile;
+  int ring_max;
+  const int32_t* tile_meta;
+  const int32_t* runs;
+  const uint16_t* local;
+} gsp_ring_plan;
+int gsp_cheby_ring_plan_host(int64_t n, const int32_t* indptr_host, const int32_t* indices_host,
+                             int rows_per_tile, int64_t run_capacity, int32_t* tile_meta,
+                             int32_t* runs, uint16_t* local, int64_t* run_count_out,
+                             int32_t* ring_max_out);
+int gsp_cheby_ring_fits(int ring_max, int64_t nsig, const gsp_tile_plan* plan_host);
+int gsp_cheby_clenshaw_ring_f32(int64_t n, int64_t nnz, const int32_t* indptr,
+                                const int32_t* indices, const float* data, double lmax,
+                                const double* coeffs_host, int nsrc, int m, const float* sources,
+                                int64_t nsig, float* out, float* work,
+                                const gsp_tile_plan* plan_host, const gsp_ring_plan* ring_host,
+                                const int32_t* slots_fwd, const int32_t* slots_rev,
+                                const int32_t* nbr_ptr, const int32_t* nbr_idx,
+                                uint32_t* tile_done, void* stream);
 int gsp_cheby_clenshaw_pairs_f32(int64_t n, int64_t nnz, const int32_t* indptr,
                                  const int32_t* indices, const float* data, double lmax,
                                  const double* coeffs_host, int m, const float* source,

@@ -30,6 +30,12 @@ class TilePlan(ctypes.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_}
 
 
+class RingPlan(ctypes.Structure):
+    """Mirror of ``gsp_ring_plan`` (include/gspb200.h)."""
+    _fields_ = [("rows_per_tile", ctypes.c_int), ("ring_max", ctypes.c_int),
+                ("tile_meta", ctypes.c_void_p), ("runs", ctypes.c_void_p), ("local", ctypes.c_void_p)]
+
+
 class HaloFusion(ctypes.Structure):
     """Mirror of ``gsp_halo_fusion`` (include/gspb200.h)."""
     _fields_ = [("n_push_rows", ctypes.c_int64), ("n_push_tiles", ctypes.c_int64),
@@ -101,7 +107,7 @@ def _arg(a):
     """torch tensor -> device pointer; None -> NULL; numpy -> host pointer."""
     if a is None:
         return ctypes.c_void_p(0)
-    if isinstance(a, (TilePlan, HaloFusion, DistPlan)):
+    if isinstance(a, (TilePlan, RingPlan, HaloFusion, DistPlan)):
         return ctypes.byref(a)
     if hasattr(a, "data_ptr"):
         return ctypes.c_void_p(a.data_ptr())

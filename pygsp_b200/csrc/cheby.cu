@@ -365,7 +365,7 @@ template <typename T>
 int cheby_clenshaw(int64_t n, int64_t nnz, const int32_t* indptr, const int32_t* indices,
                    const T* vals, double lmax, const double* c, int nsrc, int m, const T* src,
                    int nsig, T* out, T* work, const gsp_tile_plan* plan, cudaStream_t st,
-                   const ClenshawPairs* pairs = nullptr) {
+                   const ClenshawPairs* pairs = nullptr, const gsp_ring_plan* ring = nullptr) {
   GSP_REQUIRE(n >= 0 && nsig >= 1 && nsrc >= 1 && nsrc <= kMaxScales, "bad sizes");
   GSP_REQUIRE(m >= 2, "The coefficients have an invalid shape");
   GSP_REQUIRE(lmax > 0 && lmax == lmax, "lmax must be positive");
@@ -376,6 +376,7 @@ int cheby_clenshaw(int64_t n, int64_t nnz, const int32_t* indptr, const int32_t*
   Step<T> s{nnz, indptr, indices, vals};
   s.r_rows = n;
   s.nsig = nsig;
+  s.ring = ring;
   const T* b_cur = buf[0];
   const T* b_old = nullptr;
   int k_next;
@@ -550,14 +551,23 @@ int gsp_cheby_clenshaw_pairs_wanted(int64_t n, int64_t nsig, const gsp_tile_plan
   return n * nsig * int64_t(sizeof(float)) > int64_t(l2);
 }
 
-int gsp_cheby_clenshaw_pairs_f32(int64_t n, int64_t nnz, const int32_t* indptr,
-                                 const int32_t* indices, const float* data, double lmax,
-                                 const double* coeffs_host, int m, const float* source,
-                                 int64_t nsig, float* out, float* work,
-                                 const gsp_tile_plan* plan_host, const int32_t* slots_fwd,
-                                 const int32_t* slots_rev, const int32_t* nbr_ptr,
-                                 const int32_t* nbr_idx, uint32_t* tile_done, void* stream) {
+int gsp_cheby_clenshaw_ring_f32(int64_t n, int64_t nnz, const int32_t* indptr,
+                                const int32_t* indices, const float* data, double lmax,
+                                const double* coeffs_host, int nsrc, int m, const float* sources,
+                                int64_t nsig, float* out, float* work,
+                                const gsp_tile_plan* plan_host, const gsp_ring_plan* ring_host,
+                                const int32_t* slots_fwd, const int32_t* slots_rev,
+                                const int32_t* nbr_ptr, const int32_t* nbr_idx,
+                                uint32_t* tile_done, void* stream) {
   GSP_REQUIRE(nsig >= 1 && nsig <= (1 << 20), "nsig out of range");
+  GSP_REQUIRE(!ring_host || (plan_host && ring_host->rows_per_tile == plan_host->rows_per_tile &&
+                             ring_host->tile_meta && ring_host->runs && ring_host->local),
+              "the ring plan must be one of the tile plan's rows per tile");
+  if (!slots_fwd)
+    return gsp::cheby_clenshaw<float>(n, nnz, indptr, indices, data, lmax, coeffs_host, nsrc, m,
+                                      sources, (int)nsig, out, work, plan_host,
+                                      gsp::as_stream(stream), nullptr, ring_host);
+  GSP_REQUIRE(nsrc == 1, "paired steps take one source");
   GSP_REQUIRE(plan_host && plan_host->rows_per_tile > 0, "paired steps need a tile plan");
   GSP_REQUIRE(slots_fwd && slots_rev && nbr_ptr && nbr_idx && tile_done,
               "paired steps need a pair plan");
@@ -565,13 +575,27 @@ int gsp_cheby_clenshaw_pairs_f32(int64_t n, int64_t nnz, const int32_t* indptr,
   probe.x_cur = work;
   probe.x_old = work + n * nsig;
   probe.x_new = work + 2 * n * nsig;
-  probe.r = const_cast<float*>(source);
+  probe.r = const_cast<float*>(sources);
   probe.nscales = 1;
   GSP_REQUIRE(gsp::tiled_step_applies(probe, 0, plan_host) && gsp::aligned16(out),
               "paired steps need 16-byte aligned blocks");
   const gsp::ClenshawPairs pairs{slots_fwd, slots_rev, nbr_ptr, nbr_idx, tile_done};
-  return gsp::cheby_clenshaw<float>(n, nnz, indptr, indices, data, lmax, coeffs_host, 1, m, source,
-                                    (int)nsig, out, work, plan_host, gsp::as_stream(stream), &pairs);
+  return gsp::cheby_clenshaw<float>(n, nnz, indptr, indices, data, lmax, coeffs_host, 1, m,
+                                    sources, (int)nsig, out, work, plan_host,
+                                    gsp::as_stream(stream), &pairs, ring_host);
+}
+
+int gsp_cheby_clenshaw_pairs_f32(int64_t n, int64_t nnz, const int32_t* indptr,
+                                 const int32_t* indices, const float* data, double lmax,
+                                 const double* coeffs_host, int m, const float* source,
+                                 int64_t nsig, float* out, float* work,
+                                 const gsp_tile_plan* plan_host, const int32_t* slots_fwd,
+                                 const int32_t* slots_rev, const int32_t* nbr_ptr,
+                                 const int32_t* nbr_idx, uint32_t* tile_done, void* stream) {
+  GSP_REQUIRE(slots_fwd, "paired steps need a pair plan");
+  return gsp_cheby_clenshaw_ring_f32(n, nnz, indptr, indices, data, lmax, coeffs_host, 1, m,
+                                     source, nsig, out, work, plan_host, nullptr, slots_fwd,
+                                     slots_rev, nbr_ptr, nbr_idx, tile_done, stream);
 }
 
 int gsp_cheby_step_halo_f32(int first, int64_t n_rows, int64_t nnz, const int32_t* indptr,

@@ -17,6 +17,10 @@
 //     order, apply the three-term recurrence and the coefficient AXPYs and store
 //     x_new / r with streaming 16-byte stores; then release the stage ("empty").
 //
+// With neighbour rings (single-source Clenshaw steps whose rings fit, RING instantiations) the
+// producer warp also copies the tile's ring -- the x_cur rows its rows reference, and its own --
+// into the stage, and the gather reads shared memory (stage_ring_tile, DESIGN.md section 4.1).
+//
 // Two optional roles of the same kernel:
 //   * add_source (Clenshaw form): the r tiles are read-only source blocks,
 //     x_new += sum_i ck_i s_i, nothing is written to r  (single-filter Clenshaw and
@@ -78,6 +82,13 @@ struct TileArgs {
   const float* x_old2 = nullptr;
   float* x_new2 = nullptr;
   float ck2 = 0.f;
+  // Neighbour rings (gsp_ring_plan; ring_cap == 0: none).  The producer copies tile t's ring rows
+  // of the gathered block into the stage, and the CSR slab carries ring positions (ring_local)
+  // instead of column ids.  Only with row_begin == 0, a stage without vector tiles and no halo.
+  const int4* ring_meta = nullptr;     // per tile: first run, end of runs, ring rows, position of row t R
+  const int2* ring_runs = nullptr;     // per run: first row, ring position
+  const uint16_t* ring_local = nullptr;
+  int ring_cap = 0;                    // ring rows a stage holds
 };
 
 // ----------------------------------------------------------------- PTX helpers
@@ -146,17 +157,22 @@ __device__ __forceinline__ void store_f4(float* p, const float4& v, bool keep) {
 }
 
 // shared-memory carve-up, identical on host and device
+// Without a ring a stage is [vector tiles | column ids | values | indptr]; with one (no vector
+// tiles then) it is [ring rows | values | ring positions | indptr].
 struct TileLayout {
-  int vec_bytes;      // x_old + r tiles of one stage
-  int slab_bytes;     // one of the two CSR slabs
+  int vec_bytes;      // x_old + r tiles of one stage, or the ring rows
+  int slab_bytes;     // the values slab (4-byte column ids: as large, 2-byte ring positions: half)
+  int idx_bytes;
   int ptr_bytes;      // indptr slab + trailing slot
   int stage_bytes;
   int bar_bytes;
-  __host__ __device__ TileLayout(int R, int cap, int nsig, int nscales, bool first, int stages) {
-    vec_bytes = first ? 0 : (1 + nscales) * R * nsig * 4;
+  __host__ __device__ TileLayout(int R, int cap, int nsig, int nscales, bool first, int stages,
+                                 int ring_cap = 0) {
+    vec_bytes = ring_cap ? ring_cap * nsig * 4 : (first ? 0 : (1 + nscales) * R * nsig * 4);
     slab_bytes = (cap + 16) * 4;                // +16: aligned groups may run past the end
+    idx_bytes = ring_cap ? slab_bytes / 2 : slab_bytes;
     ptr_bytes = (R + 4) * 4;
-    stage_bytes = vec_bytes + 2 * slab_bytes + ptr_bytes + 16;   // +16: slab offset, group counter
+    stage_bytes = vec_bytes + slab_bytes + idx_bytes + ptr_bytes + 16;   // +16: slab offset, ring position of the tile
     bar_bytes = ((2 * stages * 8 + 15) / 16) * 16;
   }
   __host__ __device__ int total(int stages) const { return bar_bytes + stages * stage_bytes; }
@@ -186,13 +202,26 @@ __device__ __forceinline__ float4 ld_plain_f4(const float* p) {
                : "l"(p));
   return v;
 }
-constexpr int kGatherNc = 0, kGatherL2 = 1, kGatherPlain = 2;
+// kGatherRing: the rows come from the tile's neighbour ring in shared memory, `col` is a ring
+// position.
+constexpr int kGatherNc = 0, kGatherL2 = 1, kGatherPlain = 2, kGatherRing = 3;
 template <int COH>
 __device__ __forceinline__ float4 gather_f4(const float* __restrict__ xg, int col, int ns) {
+  if (COH == kGatherRing) return *reinterpret_cast<const float4*>(xg + col * ns);
   const float* p = xg + int64_t(col) * ns;
   if (COH == kGatherL2) return __ldcg(reinterpret_cast<const float4*>(p));
   if (COH == kGatherPlain) return ld_plain_f4(p);
   return ldg_f4(p);
+}
+
+// four column ids (one LDS.128) or four 16-bit ring positions (one LDS.64) of an aligned group
+__device__ __forceinline__ void load_idx4(const int32_t* p, int (&c)[4]) {
+  const int4 v = *reinterpret_cast<const int4*>(p);
+  c[0] = v.x; c[1] = v.y; c[2] = v.z; c[3] = v.w;
+}
+__device__ __forceinline__ void load_idx4(const uint16_t* p, int (&c)[4]) {
+  const uint2 v = *reinterpret_cast<const uint2*>(p);
+  c[0] = int(v.x & 0xffffu); c[1] = int(v.x >> 16); c[2] = int(v.y & 0xffffu); c[3] = int(v.y >> 16);
 }
 
 // sum_j w_j x_cur[col_j, packets of this lane] over the stored entries [jb, je) of one row
@@ -206,8 +235,8 @@ __device__ __forceinline__ float4 gather_f4(const float* __restrict__ xg, int co
 // are in flight per lane at a time (the same 64 bytes either way).
 // COH: the row may reference halo columns (boundary tiles of a partitioned step) -- the tile
 // gathers through L2 then; interior tiles use the plain non-coherent gather only.
-template <int G, int P, int COH>
-__device__ __forceinline__ void row_gather_sum(const int32_t* __restrict__ sm_col,
+template <int G, int P, int COH, typename IDX>
+__device__ __forceinline__ void row_gather_sum(const IDX* __restrict__ sm_col,
                                                const float* __restrict__ sm_val, int jb, int je,
                                                const float* __restrict__ xg, float4 (&acc)[P]) {
   constexpr int NS = 4 * G * P;
@@ -216,10 +245,10 @@ __device__ __forceinline__ void row_gather_sum(const int32_t* __restrict__ sm_co
 #pragma unroll
   for (int p = 0; p < P; ++p) acc[p] = make_float4(0.f, 0.f, 0.f, 0.f);
   for (int jj = jb & ~3; jj < je; jj += 4) {
-    const int4 c4 = *reinterpret_cast<const int4*>(sm_col + jj);
+    int cq[4];
+    load_idx4(sm_col + jj, cq);
     const float4 w4 = *reinterpret_cast<const float4*>(sm_val + jj);
     const int base = jj - jb;
-    const int cq[4] = {c4.x, c4.y, c4.z, c4.w};
     const float wq[4] = {w4.x, w4.y, w4.z, w4.w};
 #pragma unroll
     for (int h = 0; h < P; ++h) {
@@ -251,10 +280,11 @@ __device__ __forceinline__ void row_gather_sum(const int32_t* __restrict__ sm_co
 
 // What a consumer lane needs to process one staged tile.
 struct TileCtx {
-  const float* sm_vec;      // x_old tile, then one r / source tile per scale (empty in direct mode)
-  const int32_t* sm_col;    // CSR slab: column indices
+  const float* sm_vec;      // x_old tile, then one r / source tile per scale (empty in direct
+                            // mode); with a ring: the ring rows
+  const void* sm_col;       // CSR slab: column indices (int32), with a ring ring positions (uint16)
   const float* sm_val;      //           values
-  const int32_t* sm_ptr;    // indptr[r0 .. r0 + R], slab offset at [R + 4]
+  const int32_t* sm_ptr;    // indptr[r0 .. r0 + R], slab offset at [R + 4], ring position of r0 at [R + 5]
   int64_t tile;
   int64_t r0;               // first row of the tile (block-local row index)
   int cw, sub, c0;          // consumer warp, row slot inside the warp, first column of the lane
@@ -270,6 +300,7 @@ __device__ __forceinline__ void fma4(float4& d, float w, const float4& v) {
 
 // The rows of one tile: gather + three-term recurrence + coefficient AXPYs + stores.
 // COH: the tile's rows may reference halo columns (coherent gathers through L2).
+// COH == kGatherRing: the x_cur rows (the gathered ones and the tile's own) come from the ring.
 // PAIR (paired launch): 1 = step A, 2 = step B.  B takes its blocks and ck from the second operand
 // set and reads the gathered block, which A writes in the same launch, with plain loads.  A reads
 // the source rows through L2 without the evict-first mark, since B reads them again.
@@ -284,7 +315,9 @@ __device__ __forceinline__ void tile_rows(const TileArgs& a, const TileCtx t) {
   const int R = a.rows_per_tile;
   const int NW = a.consumer_warps;
   const int c0 = t.c0;
-  const float* __restrict__ xg = x_cur_blk + c0;    // this lane's first column packet of x_cur
+  constexpr bool RING = COH == kGatherRing;
+  // this lane's first column packet of x_cur, or of the ring
+  const float* __restrict__ xg = (RING ? t.sm_vec : x_cur_blk) + c0;
   const int nscales = NSC >= 0 ? NSC : a.nscales;
   const float alpha = a.alpha, beta = a.beta, gamma = a.gamma;
   // (B's stores are evict-first: nothing reads them before the next launch, and L2 is what the
@@ -294,7 +327,7 @@ __device__ __forceinline__ void tile_rows(const TileArgs& a, const TileCtx t) {
   const float* sm_vec = t.sm_vec;
   const int a0 = t.sm_ptr[R + 4];
   const int64_t r0 = t.r0;
-  const float* __restrict__ xc_tile = xg + r0 * NS;
+  const float* __restrict__ xc_tile = xg + (RING ? int64_t(t.sm_ptr[R + 5]) : r0) * NS;
   float* __restrict__ xn_tile = x_new_blk + r0 * NS + c0;
   float* __restrict__ r_tile = a.r + r0 * NS + c0;
   const int64_t r_stride = a.r_rows * NS;
@@ -306,7 +339,9 @@ __device__ __forceinline__ void tile_rows(const TileArgs& a, const TileCtx t) {
     float4 xc[P];
 #pragma unroll
     for (int p = 0; p < P; ++p)
-      xc[p] = COH == kGatherPlain ? ld_plain_f4(xc_tile + off + p * PS) : ldg_f4(xc_tile + off + p * PS);
+      xc[p] = COH == kGatherPlain ? ld_plain_f4(xc_tile + off + p * PS)
+              : RING ? *reinterpret_cast<const float4*>(xc_tile + off + p * PS)
+                     : ldg_f4(xc_tile + off + p * PS);
     // direct mode: this row's x_old and first r / source packets are requested now (streaming
     // loads, no L1 allocation) and consumed after the gather loop, which hides their latency
     float4 xo_d[P], r0_d[P];
@@ -323,7 +358,10 @@ __device__ __forceinline__ void tile_rows(const TileArgs& a, const TileCtx t) {
       }
     }
     float4 acc[P];
-    row_gather_sum<G, P, COH>(t.sm_col, t.sm_val, jb, je, xg, acc);
+    if constexpr (RING)
+      row_gather_sum<G, P, COH>(static_cast<const uint16_t*>(t.sm_col), t.sm_val, jb, je, xg, acc);
+    else
+      row_gather_sum<G, P, COH>(static_cast<const int32_t*>(t.sm_col), t.sm_val, jb, je, xg, acc);
     float4 xn[P];
 #pragma unroll
     for (int p = 0; p < P; ++p) {
@@ -456,18 +494,68 @@ __device__ __noinline__ void boundary_tile(const TileArgs& a, const TileCtx t, i
   }
 }
 
+// Ring mode, the whole producer warp: stage tile `tile` (CSR entries [begin, end), ring `m`) in
+// stage `st` -- indptr, values and ring positions by lane 0, then one bulk copy of the rows of
+// `xg` per run of the ring, spread over the lanes.  One expect_tx covers the stage.  The slab
+// starts at a multiple of 8 entries, so that the 2-byte positions are 16-byte aligned as well.
+__device__ __forceinline__ void stage_ring_tile(const TileArgs& a, const TileLayout& lay,
+                                                unsigned char* st, uint64_t* full, int64_t tile,
+                                                int begin, int end, int4 m, const float* xg,
+                                                bool evict, uint64_t pol, int lane) {
+  const int R = a.rows_per_tile;
+  const int nsig = a.nsig;
+  float* sm_ring = reinterpret_cast<float*>(st);
+  float* sm_val = reinterpret_cast<float*>(st + lay.vec_bytes);
+  uint16_t* sm_loc = reinterpret_cast<uint16_t*>(st + lay.vec_bytes + lay.slab_bytes);
+  int32_t* sm_ptr = reinterpret_cast<int32_t*>(st + lay.vec_bytes + lay.slab_bytes + lay.idx_bytes);
+  const uint32_t row_bytes = uint32_t(nsig) * 4u;
+  if (lane == 0) {
+    const int64_t r0 = tile * R;
+    const int a0 = begin & ~7;
+    int a1 = (end + 7) & ~7;
+    if (int64_t(a1) > a.nnz) a1 = end & ~7;     // never read past the arrays
+    sm_ptr[R] = end;                            // the bulk copy brings indptr[r0 .. r0+R)
+    sm_ptr[R + 4] = a0;
+    sm_ptr[R + 5] = m.w;
+    for (int k = (a1 > a0 ? a1 : a0); k < end; ++k) {   // <= 7 trailing entries, last tile only
+      sm_val[k - a0] = __ldg(a.vals + k);
+      sm_loc[k - a0] = __ldg(a.ring_local + k);
+    }
+    const uint32_t len = a1 > a0 ? uint32_t(a1 - a0) : 0u;
+    mbar_expect_tx(full, uint32_t(R) * 4u + 6u * len + uint32_t(m.z) * row_bytes);
+    bulk_g2s(sm_ptr, a.indptr + r0, uint32_t(R) * 4u, full);
+    if (len && evict) {
+      bulk_g2s_hint(sm_val, a.vals + a0, 4u * len, full, pol);
+      bulk_g2s_hint(sm_loc, a.ring_local + a0, 2u * len, full, pol);
+    } else if (len) {
+      bulk_g2s(sm_val, a.vals + a0, 4u * len, full);
+      bulk_g2s(sm_loc, a.ring_local + a0, 2u * len, full);
+    }
+  }
+  __syncwarp();                                 // the expect_tx precedes every complete_tx
+  for (int i = m.x + lane; i < m.y; i += 32) {
+    const int2 run = __ldg(a.ring_runs + i);
+    const int next = i + 1 < m.y ? __ldg(a.ring_runs + i + 1).y : m.z;
+    bulk_g2s(sm_ring + size_t(run.y) * nsig, xg + int64_t(run.x) * nsig,
+             uint32_t(next - run.y) * row_bytes, full);
+  }
+}
+
 // One packet per lane: 1 + 16 warps per CTA, 2 CTAs per SM (<= 60 registers).  Two packets per
 // lane keep twice the state per lane: 1 + 8 warps, 3 CTAs per SM (<= 75 registers).
-template <int G, bool FIRST, int NSC, bool HALO, int P>
+// RING: the gather reads the tile's neighbour ring, staged by the whole producer warp (no halo,
+// first step or direct vectors).
+template <int G, bool FIRST, int NSC, bool HALO, int P, bool RING>
 __global__ void __launch_bounds__(32 * (P == 2 ? 9 : 17), P == 2 ? 3 : 2)
 cheby_step_tiled(const __grid_constant__ TileArgs a) {
+  static_assert(!(RING && HALO), "the halo path keeps the gather from global memory");
   extern __shared__ __align__(128) unsigned char smem[];
   const int R = a.rows_per_tile;
   const int S = a.stages;
   const int NW = a.consumer_warps;
   const int nsig = a.nsig;
   const bool VD = !FIRST && a.vec_direct != 0;     // CTA-uniform
-  const TileLayout lay(R, a.slab_cap, nsig, a.nscales, FIRST || VD, S);
+  const TileLayout lay(R, a.slab_cap, nsig, a.nscales, FIRST || VD, S, RING ? a.ring_cap : 0);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem);
   uint64_t* empty = full + S;
   unsigned char* stage0 = smem + lay.bar_bytes;
@@ -487,11 +575,24 @@ cheby_step_tiled(const __grid_constant__ TileArgs a) {
   if (warp == 0) {
     // ------------------------------------------------------------- producer
     // (nothing the producer stages depends on the halo: CSR slabs, x_old and r rows are local)
-    if (lane != 0) return;
     // x_old / r / CSR are touched once per step: mark them evict-first so that the
     // L2 keeps the x_cur lines the gathers re-use (GSPB200_TILE_HINT=0 disables)
     const bool hint = a.l2_hint != 0;
     const uint64_t pol = l2_policy_evict_first();
+    if (RING) {
+      int it = 0;
+      for (int64_t slot = blockIdx.x; slot < a.n_tiles; slot += gridDim.x, ++it) {
+        const int64_t tile = tile_of_slot(a, slot);
+        const int begin = __ldg(a.indptr + tile * R), end = __ldg(a.indptr + tile * R + R);
+        const int4 m = __ldg(a.ring_meta + tile);
+        const int s = it % S;
+        mbar_wait(empty + s, (uint32_t(it / S) & 1u) ^ 1u);
+        stage_ring_tile(a, lay, stage0 + size_t(s) * lay.stage_bytes, full + s, tile, begin, end,
+                        m, a.x_cur, hint, pol, lane);
+      }
+      return;
+    }
+    if (lane != 0) return;
     int it = 0;
     // the tile's first / last CSR offsets are fetched one tile ahead, so that their
     // DRAM latency is not in series with the wait for a free slot
@@ -576,15 +677,17 @@ cheby_step_tiled(const __grid_constant__ TileArgs a) {
     unsigned char* st = stage0 + size_t(s) * lay.stage_bytes;
     // (the context is built per use and passed BY VALUE: a struct whose address escapes to the
     //  non-inlined boundary routine would live in local memory for the interior path too)
-    const TileCtx t = {reinterpret_cast<const float*>(st),
-                       reinterpret_cast<const int32_t*>(st + lay.vec_bytes),
-                       reinterpret_cast<const float*>(st + lay.vec_bytes + lay.slab_bytes),
-                       reinterpret_cast<const int32_t*>(st + lay.vec_bytes + 2 * lay.slab_bytes),
+    // (ring: [ring | values | positions | indptr], else [vectors | columns | values | indptr])
+    const unsigned char* sl0 = st + lay.vec_bytes;
+    const unsigned char* sl1 = sl0 + lay.slab_bytes;
+    const TileCtx t = {reinterpret_cast<const float*>(st), RING ? sl1 : sl0,
+                       reinterpret_cast<const float*>(RING ? sl0 : sl1),
+                       reinterpret_cast<const int32_t*>(sl1 + lay.idx_bytes),
                        tile, a.row_begin + tile * R, cw, sub, c0, VD};
     if (HALO && tile < a.n_front)          // warp-uniform; interior tiles never wait
       boundary_tile<G, FIRST, NSC>(a, t, lane);
     else
-      tile_rows<G, FIRST, NSC, kGatherNc, P>(a, t);
+      tile_rows<G, FIRST, NSC, RING ? kGatherRing : kGatherNc, P>(a, t);
     __syncwarp();
     if (lane == 0) mbar_arrive(empty + s);
   }
@@ -601,21 +704,39 @@ cheby_step_tiled(const __grid_constant__ TileArgs a) {
 // read-only, W is written by A and read by B only, and the rows of Q that B(t) overwrites are
 // read by A(t) alone.  Per row the instructions are those of the single step: the same bits.
 //
-// An acquire at GPU scope makes the SM drop its L1 (CCTL.IVALL), which the gathers of all resident
-// CTAs live on, so it is paid once per B tile and CTA and never inside a poll loop: consumer warp
-// 0 polls with relaxed loads, fences once, and a named barrier hands the tile to the other
-// consumer warps.  On the release side each warp's stores are ordered by __syncwarp before lane
-// 0's red.release (a fence without L1 invalidation).
-template <int G, int P>
+// On the release side each warp's stores are ordered by __syncwarp before lane 0's red.release (a
+// fence without L1 invalidation).  The acquire side has two forms.
+//
+// RING (the neighbour rings fit): A(t) stages the ring of P, B(t) the ring of W, and the producer
+// warp waits for B(t)'s A tiles before it stages B(t), while the consumers still work on the slots
+// before it: its lanes poll the flags with relaxed loads, then every lane issues
+// fence.acq_rel.gpu -- with the relaxed reads of the flags and the releasing red of the A warps
+// this is the fence-based release / acquire pattern that makes A's stores of W visible (PTX ISA,
+// "Memory Consistency Model", sections on release / acquire patterns and causality order) -- and
+// fence.proxy.async.global, which orders those generic-proxy stores before the async-proxy reads
+// of the bulk copies that follow (same chapter, "Proxies").  The consumers see the staged rows
+// through the stage's mbarrier.  Nothing the gathers read lives in L1, so the L1 invalidation that
+// the acquire implies costs nothing.  No deadlock: the producer stages its CTA's slots in order,
+// at most `stages` ahead of the consumers; an A slot waits for nothing, a B slot only for A slots
+// lower in the table (checked when the table is built); so the lowest unfinished slot of the
+// launch -- whose CTA has finished, and so has freed the stages of, every slot before it -- can
+// always be staged and run, given that every CTA of the grid is resident (the launch requires it).
+//
+// Without a ring, the gathers of all resident CTAs live on L1, so the acquire is paid once per B
+// tile and CTA and never inside a poll loop: consumer warp 0 polls with relaxed loads, fences once,
+// and a named barrier hands the tile to the other consumer warps (one stage).
+template <int G, int P, bool RING>
 __global__ void __launch_bounds__(32 * (P == 2 ? 9 : 17), P == 2 ? 3 : 2)
 cheby_pair_tiled(const __grid_constant__ TileArgs a) {
   extern __shared__ __align__(128) unsigned char smem[];
   const int R = a.rows_per_tile;
   const int NW = a.consumer_warps;
-  const TileLayout lay(R, a.slab_cap, a.nsig, a.nscales, true, 1);
+  const int S = RING ? a.stages : 1;
+  const TileLayout lay(R, a.slab_cap, a.nsig, a.nscales, true, S, RING ? a.ring_cap : 0);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem);
-  uint64_t* empty = full + 1;
-  unsigned char* st = smem + lay.bar_bytes;
+  uint64_t* empty = full + S;
+  unsigned char* stage0 = smem + lay.bar_bytes;
+  unsigned char* st = stage0;
   int32_t* sm_col = reinterpret_cast<int32_t*>(st);
   float* sm_val = reinterpret_cast<float*>(st + lay.slab_bytes);
   int32_t* sm_ptr = reinterpret_cast<int32_t*>(st + 2 * lay.slab_bytes);
@@ -623,11 +744,77 @@ cheby_pair_tiled(const __grid_constant__ TileArgs a) {
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
-    mbar_init(full, 1);
-    mbar_init(empty, NW);
+    for (int s = 0; s < S; ++s) {
+      mbar_init(full + s, 1);
+      mbar_init(empty + s, NW);
+    }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
+
+  if (RING && warp == 0) {
+    const uint64_t pol = l2_policy_evict_first();
+    uint32_t it = 0;
+    for (int64_t slot = blockIdx.x; slot < a.n_slots; slot += gridDim.x, ++it) {
+      const int code = __ldg(a.slots + slot);
+      const int64_t tile = code >> 1;
+      const int begin = __ldg(a.indptr + tile * R), end = __ldg(a.indptr + tile * R + R);
+      const int4 m = __ldg(a.ring_meta + tile);
+      if (code & 1) {
+        // the wait of B(tile); bounded all the same: a wait of seconds can only be a broken table,
+        // and a trapped launch is reported to the caller where a spinning one would hold the device
+        const int e1 = __ldg(a.nbr_ptr + tile + 1);
+        for (int e = __ldg(a.nbr_ptr + tile) + lane; e < e1; e += 32) {
+          const unsigned* f = a.tile_done + __ldg(a.nbr_idx + e);
+          unsigned seen, polls = 0;
+          for (;;) {
+            asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(seen) : "l"(f) : "memory");
+            if (seen >= a.done_target) break;
+            if (++polls > (1u << 24)) __trap();
+            __nanosleep(128);
+          }
+        }
+        __syncwarp();
+        asm volatile("fence.acq_rel.gpu;" ::: "memory");
+        asm volatile("fence.proxy.async.global;" ::: "memory");
+      }
+      const int s = int(it % uint32_t(S));
+      mbar_wait(empty + s, ((it / uint32_t(S)) & 1u) ^ 1u);
+      // A's slab stays in L2 for B(t): 12.16 -> 12.02 ms
+      stage_ring_tile(a, lay, stage0 + size_t(s) * lay.stage_bytes, full + s, tile, begin, end, m,
+                      (code & 1) ? a.x_cur2 : a.x_cur, a.l2_hint != 0 && (code & 1), pol, lane);
+    }
+    return;
+  }
+  if (RING) {
+    const int cw = warp - 1;
+    const int sub = lane / G;
+    const int c0 = (lane % G) * 4;
+    uint32_t it = 0;
+    for (int64_t slot = blockIdx.x; slot < a.n_slots; slot += gridDim.x, ++it) {
+      const int code = __ldg(a.slots + slot);
+      const int64_t tile = code >> 1;
+      const int s = int(it % uint32_t(S));
+      mbar_wait(full + s, (it / uint32_t(S)) & 1u);
+      const unsigned char* sg = stage0 + size_t(s) * lay.stage_bytes;
+      const TileCtx t = {reinterpret_cast<const float*>(sg), sg + lay.vec_bytes + lay.slab_bytes,
+                         reinterpret_cast<const float*>(sg + lay.vec_bytes),
+                         reinterpret_cast<const int32_t*>(sg + lay.vec_bytes + lay.slab_bytes +
+                                                          lay.idx_bytes),
+                         tile, tile * R, cw, sub, c0, true};
+      if (code & 1) {
+        tile_rows<G, false, 1, kGatherRing, P, 2>(a, t);
+      } else {
+        tile_rows<G, false, 1, kGatherRing, P, 1>(a, t);
+        __syncwarp();
+        if (lane == 0)
+          asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(a.tile_done + tile) : "memory");
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty + s);
+    }
+    return;
+  }
 
   if (warp == 0) {
     // producer: the CSR slab of the slot's tile (the same slab for A(t) and B(t)); the slot table
@@ -790,14 +977,33 @@ int tile_plan(int64_t n, const int32_t* indptr, int64_t nsig, int nscales, gsp_t
   return GSP_OK;
 }
 
-template <int G, int NSC, bool HALO, int P>
+// Stages of a step with neighbour rings of up to ring_max rows: as many as the shared-memory
+// budget of a CTA holds, at most GSPB200_RING_S (default kRingStages); 0 when not even one fits.
+// The budget lets two CTAs share an SM (2 x (113 + 1) KB of 228 KB).  Measured on an H100 SXM
+// (700 W), config 2 of bench.py (1e6-vertex Morton k-NN, 64 signals, order 30, R = 64, largest
+// ring 178 rows, a stage of about 54 KB): one stage and three CTAs per SM 10.12 ms per call, two
+// stages and two CTAs per SM 9.68 ms; R = 32 12.15 ms, R = 128 10.87 ms (DESIGN.md section 4.1).
+constexpr int kRingStages = 2;
+constexpr int kRingBudget = 113 * 1024;
+static int ring_stages(const gsp_tile_plan& plan, int nsig, int ring_max) {
+  if (plan.rows_per_tile <= 0 || ring_max <= 0 || env_int("GSPB200_TILE_RING", 1) == 0) return 0;
+  const int budget = env_int("GSPB200_RING_SMEM", kRingBudget);
+  for (int s = std::max(1, env_int("GSPB200_RING_S", kRingStages)); s >= 1; --s)
+    if (TileLayout(plan.rows_per_tile, plan.slab_capacity, nsig, 0, true, s, ring_max).total(s) <=
+        budget)
+      return s;
+  return 0;
+}
+
+template <int G, int NSC, bool HALO, int P, bool RING = false>
 static int launch_tiled_k(bool first, const TileArgs& a, int blocks_per_sm, cudaStream_t st) {
   const TileLayout lay(a.rows_per_tile, a.slab_cap, a.nsig, a.nscales, first || a.vec_direct,
-                       a.stages);
+                       a.stages, a.ring_cap);
   const int smem = lay.total(a.stages);
   const int threads = 32 * (1 + a.consumer_warps);
   GSP_REQUIRE(threads <= 32 * (P == 2 ? 9 : 17), "too many consumer warps for this mapping");
-  auto kern = first ? cheby_step_tiled<G, true, NSC, HALO, P> : cheby_step_tiled<G, false, NSC, HALO, P>;
+  auto kern = first ? cheby_step_tiled<G, true, NSC, HALO, P, RING>
+                    : cheby_step_tiled<G, false, NSC, HALO, P, RING>;
   GSP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   int per_sm = 0;
   GSP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem));
@@ -811,6 +1017,11 @@ static int launch_tiled_k(bool first, const TileArgs& a, int blocks_per_sm, cuda
 
 template <int G, bool HALO, int P>
 static int launch_tiled_gh(bool first, const TileArgs& a, int bps, cudaStream_t st) {
+  if constexpr (!HALO) {
+    // rings: the single-source Clenshaw steps (the first one has no source block)
+    if (a.ring_cap && a.nscales == 0) return launch_tiled_k<G, 0, false, P, true>(first, a, bps, st);
+    if (a.ring_cap && a.nscales == 1) return launch_tiled_k<G, 1, false, P, true>(first, a, bps, st);
+  }
   switch (a.nscales) {          // common bank widths get the scale loop unrolled
     case 0: return launch_tiled_k<G, 0, HALO, P>(first, a, bps, st);
     case 1: return launch_tiled_k<G, 1, HALO, P>(first, a, bps, st);
@@ -831,11 +1042,11 @@ static int launch_tiled_g(bool first, const TileArgs& a, bool halo, bool two, in
 
 template <int G, int P>
 static int launch_pair_k(const TileArgs& a, int blocks_per_sm, cudaStream_t st) {
-  const TileLayout lay(a.rows_per_tile, a.slab_cap, a.nsig, a.nscales, true, 1);
-  const int smem = lay.total(1);
+  const TileLayout lay(a.rows_per_tile, a.slab_cap, a.nsig, a.nscales, true, a.stages, a.ring_cap);
+  const int smem = lay.total(a.stages);
   const int threads = 32 * (1 + a.consumer_warps);
   GSP_REQUIRE(threads <= 32 * (P == 2 ? 9 : 17), "too many consumer warps for this mapping");
-  auto kern = cheby_pair_tiled<G, P>;
+  auto kern = a.ring_cap ? cheby_pair_tiled<G, P, true> : cheby_pair_tiled<G, P, false>;
   GSP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   int per_sm = 0;
   GSP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem));
@@ -907,6 +1118,19 @@ int cheby_step_tiled_f32(const Step<float>& s, int64_t rb, int64_t re, const gsp
   // than the producer running a tile ahead; the SM's other CTAs cover one CTA's wait for its TMA.
   // H100, 1e6-vertex k-NN, Clenshaw form: 14.8 -> 12.7 ms per call (DESIGN.md section 4.1).
   a.stages = (first || a.vec_direct) ? 1 : plan.stages;
+  // Neighbour rings: the gather reads shared memory only, so L1 no longer needs the room the
+  // one-stage argument above keeps for it (DESIGN.md section 4.1).
+  if (s.ring && !halo && rb == 0 && (first || a.vec_direct) && nscales <= 1 &&
+      s.ring->rows_per_tile == plan.rows_per_tile) {
+    const int rs = ring_stages(plan, nsig, s.ring->ring_max);
+    if (rs > 0) {
+      a.ring_meta = reinterpret_cast<const int4*>(s.ring->tile_meta);
+      a.ring_runs = reinterpret_cast<const int2*>(s.ring->runs);
+      a.ring_local = s.ring->local;
+      a.ring_cap = s.ring->ring_max;
+      a.stages = rs;
+    }
+  }
   a.consumer_warps = plan.consumer_warps;
   a.nsig = nsig;
   a.nscales = nscales;
@@ -964,4 +1188,9 @@ extern "C" int gsp_cheby_tile_plan(int64_t n, const int32_t* indptr, int64_t nsi
                                    gsp_tile_plan* plan_host_out, void* stream) {
   GSP_REQUIRE(plan_host_out != nullptr, "plan must not be NULL");
   return gsp::tile_plan(n, indptr, nsig, nscales, plan_host_out, gsp::as_stream(stream));
+}
+
+extern "C" int gsp_cheby_ring_fits(int ring_max, int64_t nsig, const gsp_tile_plan* plan_host) {
+  if (!plan_host || nsig < 1 || nsig > 128) return 0;
+  return gsp::ring_stages(*plan_host, int(nsig), ring_max) > 0;
 }

@@ -11,6 +11,8 @@
 // running and wait for it; the lag (in A tiles, about two slots each) puts more than one wave of
 // the grid between the two.  Either table is a topological order of "B(t) after A(s), s in
 // nbr[t]", which is verified here before a table is handed out.
+#include <algorithm>
+#include <climits>
 #include <vector>
 #include "common.cuh"
 #include "gspb200.h"
@@ -90,6 +92,69 @@ extern "C" int gsp_cheby_pair_plan_host(int64_t n, const int32_t* indptr_host,
     }
     GSP_REQUIRE(i == 2 * T && gsp::slots_are_safe(T, nbr_ptr, nbr_idx, slots),
                 "slot table is not a topological order");
+  }
+  return GSP_OK;
+}
+
+// Neighbour rings (gsp_cheby_ring_plan_host in the header).  A tile's own rows are always in its
+// ring, so they form one stretch of it and the step reads its x_cur rows there too.
+extern "C" int gsp_cheby_ring_plan_host(int64_t n, const int32_t* indptr_host,
+                                        const int32_t* indices_host, int rows_per_tile,
+                                        int64_t run_capacity, int32_t* tile_meta, int32_t* runs,
+                                        uint16_t* local, int64_t* run_count_out,
+                                        int32_t* ring_max_out) {
+  GSP_REQUIRE(n >= 0 && rows_per_tile > 0 && indptr_host && indices_host && run_count_out &&
+                  ring_max_out, "bad ring plan arguments");
+  const int64_t R = rows_per_tile, T = n / R;
+  GSP_REQUIRE(T >= 1 && T < (int64_t(1) << 30), "tile count out of range");
+  std::vector<int32_t> ring;
+  int64_t n_runs = 0, ring_max = 0;
+  for (int pass = 0; pass < 2; ++pass) {
+    // pass 0 counts; pass 1 writes, when everything fits
+    if (pass == 1) {
+      *run_count_out = n_runs;
+      *ring_max_out = int32_t(std::min<int64_t>(ring_max, INT32_MAX));
+      if (n_runs > run_capacity || ring_max > 65535) return GSP_OK;
+      GSP_REQUIRE(tile_meta && runs && local, "bad ring plan arguments");
+      const int64_t nnz = indptr_host[n];
+      for (int64_t j = indptr_host[T * R]; j < nnz; ++j) local[j] = 0;
+    }
+    std::vector<int32_t> pos(pass == 1 ? n : 0);
+    int64_t run = 0;
+    for (int64_t t = 0; t < T; ++t) {
+      ring.clear();
+      for (int64_t i = t * R; i < t * R + R; ++i) ring.push_back(int32_t(i));
+      for (int64_t j = indptr_host[t * R]; j < indptr_host[t * R + R]; ++j) {
+        GSP_REQUIRE(indices_host[j] >= 0 && indices_host[j] < n, "column index out of range");
+        ring.push_back(indices_host[j]);
+      }
+      std::sort(ring.begin(), ring.end());
+      ring.erase(std::unique(ring.begin(), ring.end()), ring.end());
+      const int64_t size = int64_t(ring.size());
+      ring_max = std::max(ring_max, size);
+      const int64_t first_run = run;
+      int64_t self = 0;
+      for (int64_t k = 0; k < size; ++k) {
+        if (k == 0 || ring[k] != ring[k - 1] + 1) {
+          if (pass == 1) {
+            runs[2 * run] = ring[k];
+            runs[2 * run + 1] = int32_t(k);
+          }
+          ++run;
+        }
+        if (ring[k] == t * R) self = k;
+        if (pass == 1) pos[ring[k]] = int32_t(k);
+      }
+      if (pass == 0) continue;
+      tile_meta[4 * t] = int32_t(first_run);
+      tile_meta[4 * t + 1] = int32_t(run);
+      tile_meta[4 * t + 2] = int32_t(size);
+      tile_meta[4 * t + 3] = int32_t(self);
+      for (int64_t j = indptr_host[t * R]; j < indptr_host[t * R + R]; ++j)
+        local[j] = uint16_t(pos[indices_host[j]]);
+    }
+    n_runs = run;
+    GSP_REQUIRE(n_runs < (int64_t(1) << 31), "too many ring runs");
   }
   return GSP_OK;
 }

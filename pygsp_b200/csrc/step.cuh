@@ -42,6 +42,7 @@ struct Step {
   bool add_source = false;
   bool reverse = false;            // tiled kernel: walk the tiles from the last to the first
   const int64_t* out_perm = nullptr;   // x_new row of local row i is out_perm[i] (NULL: i)
+  const gsp_ring_plan* ring = nullptr; // neighbour rings of the matrix (tiled kernel, rows from 0)
 };
 
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }

@@ -141,19 +141,28 @@ def cheby_clenshaw_device(L, lmax, c, sources, out=None, work=None):
     if out is None:
         out = torch.empty((n, nsig), dtype=L.dtype, device=L.device)
     plan = L.tile_plan(nsig, nsrc)
-    # one float32 source on a block larger than L2: the middle steps run two per launch, which
-    # takes a third work block (a caller's two-block work keeps the single steps)
-    if (nsrc == 1 and plan is not None and (work is None or work.shape[0] >= 3)
-            and nat.lib().gsp_cheby_clenshaw_pairs_wanted(nat.i64(n), nat.i64(nsig),
-                                                          ctypes.byref(plan))):
+    if nsrc == 1 and plan is not None:
+        # one float32 source: the tiled steps gather from each tile's neighbour ring in shared
+        # memory where the rings fit, and on a block larger than L2 the middle steps run two per
+        # launch, which takes a third work block (a caller's two-block work keeps single steps)
+        ring = L.ring_plan(plan.rows_per_tile)
+        if ring is not None and not nat.lib().gsp_cheby_ring_fits(
+                ring.ring_max, nat.i64(nsig), ctypes.byref(plan)):
+            ring = None
+        tables, tile_done = (None,) * 4, None
+        if ((work is None or work.shape[0] >= 3)
+                and nat.lib().gsp_cheby_clenshaw_pairs_wanted(nat.i64(n), nat.i64(nsig),
+                                                              ctypes.byref(plan))):
+            tables = L.pair_plan(plan.rows_per_tile)
+            tile_done = torch.empty(n // plan.rows_per_tile, dtype=torch.int32, device=L.device)
         if work is None:
-            work = torch.empty((3, n, nsig), dtype=L.dtype, device=L.device)
-        tables = L.pair_plan(plan.rows_per_tile)
-        tile_done = torch.empty(n // plan.rows_per_tile, dtype=torch.int32, device=L.device)
+            work = torch.empty((2 if tile_done is None else 3, n, nsig), dtype=L.dtype,
+                               device=L.device)
         with torch.cuda.device(L.device):
-            nat.call("gsp_cheby_clenshaw_pairs_f32", nat.i64(n), nat.i64(L.nnz), L.indptr,
-                     L.indices, L.data, nat.f64(lmax), c, nat.i32(c.shape[1]), sources,
-                     nat.i64(nsig), out, work, plan, *tables, tile_done, nat.stream_ptr(L.device))
+            nat.call("gsp_cheby_clenshaw_ring_f32", nat.i64(n), nat.i64(L.nnz), L.indptr,
+                     L.indices, L.data, nat.f64(lmax), c, nat.i32(1), nat.i32(c.shape[1]),
+                     sources, nat.i64(nsig), out, work, plan, ring, *tables, tile_done,
+                     nat.stream_ptr(L.device))
         return out
     if work is None:
         work = torch.empty((2, n, nsig), dtype=L.dtype, device=L.device)

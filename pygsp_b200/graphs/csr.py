@@ -77,6 +77,41 @@ class DeviceCSR:
                                      for a in (fwd, rev, nbr_ptr, nbr_idx[:max(count.value, 1)]))
         return self._plans[key]
 
+    def ring_plan(self, rows_per_tile):
+        """Neighbour rings of the tiled Clenshaw steps for this matrix (cached): a
+        ``_native.RingPlan`` whose device tables are those of ``gsp_cheby_ring_plan_host``,
+        which runs on a host copy of the structure.  ``ring_max`` is the largest ring; whether
+        it fits a step of ``nsig`` signals is ``gsp_cheby_ring_fits``.  None when the largest
+        ring exceeds the 16-bit ring positions."""
+        import ctypes
+        torch = nat.require_cuda()
+        key = ("rings", int(rows_per_tile))
+        if key not in self._plans:
+            indptr = self.indptr.cpu().numpy()
+            indices = self.indices.cpu().numpy()
+            n, T = self.shape[0], self.shape[0] // int(rows_per_tile)
+            count, ring_max = ctypes.c_int64(0), ctypes.c_int32(0)
+            cap = 32 * T
+            while True:
+                meta = np.empty(4 * T, dtype=np.int32)
+                runs = np.empty(2 * cap, dtype=np.int32)
+                local = np.empty(max(len(indices), 1), dtype=np.uint16)
+                nat.call("gsp_cheby_ring_plan_host", nat.i64(n), indptr, indices,
+                         nat.i32(rows_per_tile), nat.i64(cap), meta, runs, local,
+                         ctypes.byref(count), ctypes.byref(ring_max))
+                if count.value <= cap or ring_max.value > 65535:
+                    break
+                cap = count.value
+            plan = None
+            if ring_max.value <= 65535:
+                plan = nat.RingPlan(int(rows_per_tile), ring_max.value)
+                plan.tensors = tuple(torch.from_numpy(a).to(self.device)
+                                     for a in (meta, runs[:2 * max(count.value, 1)],
+                                               local.view(np.int16)))
+                plan.tile_meta, plan.runs, plan.local = (t.data_ptr() for t in plan.tensors)
+            self._plans[key] = plan
+        return self._plans[key]
+
     # -- construction ---------------------------------------------------------
     @classmethod
     def from_scipy(cls, M, dtype, device):
