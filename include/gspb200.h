@@ -845,6 +845,35 @@ int gsp_edge_resistance_f64(int64_t ne, const int32_t* erow, const int32_t* ecol
 int gsp_sparsify_sample(int64_t ne, const uint64_t* weights, int64_t q, uint64_t seed,
                         int64_t* counts, void* stream);
 
+/* ---------------------------------------------------------------- random graphs ---
+ * Draws come from Philox4x32-10 streams of `key` (curand_kernel.h) whose subsequence is a chunk
+ * id (SBM) or a slot id (BA): a graph depends on (key, parameters) only, not on the launch
+ * shape.  max_blocks caps the grid (0 = the default shape).
+ * gsp_sbm_count / gsp_sbm_fill: the pair loop of stochasticblockmodel.py:125-139 (one uniform
+ *   per vertex pair) as a Bernoulli process over each block pair's index range, walked by
+ *   geometric skips in chunks.  plan (n_blocks x GSPB200_SBM_PLAN_COLS int64, row-major, rows in
+ *   increasing cfirst) holds per block pair: n_pairs, chunk length, first global chunk id,
+ *   first position of block a and of block b in perm, nb (size of block b; n of the block for
+ *   kind 3), kind (0 rectangle, 1 strict lower triangle, 2 lower triangle with the diagonal,
+ *   3 n (n - 1) ordered pairs without the diagonal) and mirror (1: an off-diagonal pair also
+ *   emits its transpose).  prob (n_blocks x 2 double): p in (0, 1] and log1p(-p).
+ *   gsp_sbm_count writes offsets (n_chunks + 1): 0 then the inclusive scan of the entries each
+ *   chunk emits.  gsp_sbm_fill writes the COO entries (vertex ids perm[position]) of chunk c at
+ *   rows / cols [offsets[c], offsets[c + 1]).
+ * gsp_barabasi_albert: the attachment loop of barabasialbert.py:54-64.  Writes 2 m (n - m0)
+ *   COO entries, (i, v) and (v, i) for each of the m targets v of each vertex i >= m0, in
+ *   rounds of one launch each (the call synchronises the stream every few rounds);
+ *   *rounds_host_out gets the number of rounds.  -3 if the rounds do not finish.
+ */
+#define GSPB200_SBM_PLAN_COLS 8
+int gsp_sbm_count(int64_t n_chunks, int64_t n_blocks, const int64_t* plan, const double* prob,
+                  uint64_t key, int64_t* offsets, int max_blocks, void* stream);
+int gsp_sbm_fill(int64_t n_chunks, int64_t n_blocks, const int64_t* plan, const double* prob,
+                 uint64_t key, const int32_t* perm, const int64_t* offsets, int32_t* rows,
+                 int32_t* cols, int max_blocks, void* stream);
+int gsp_barabasi_albert(int64_t n, int64_t m0, int64_t m, uint64_t key, int32_t* rows,
+                        int32_t* cols, int max_blocks, int* rounds_host_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

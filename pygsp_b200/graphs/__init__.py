@@ -6,3 +6,4 @@ from .generators import (Grid2d, Grid2dImgPatches, ImgPatches, KnnSlabs, Logo,  
                          grid2d_adjacency_device, image_patches_device, knn_adjacency_device,
                          knn_device, laplacian_rows, morton_order, morton_order_device,
                          radius_device, sbm_adjacency)
+from .random_graphs import BarabasiAlbert, ErdosRenyi  # noqa: F401

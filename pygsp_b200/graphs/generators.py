@@ -802,31 +802,43 @@ def sbm_adjacency(N=1024, k=5, z=None, p=0.7, q=None, seed=None):
     return _sbm_draw(rng, N, k, z, M), z
 
 
-def _sbm_blocks(rng, N, k, z, p, q):
-    """Block assignment z (drawn from rng when None) and the k x k probability matrix M."""
+def _sbm_blocks(rng, N, k, z, p, q, M=None, sorted_z=True):
+    """Block assignment z (drawn from rng when None) and the k x k probability matrix M (built
+    from p and q unless given).  ``sorted_z``: the host sampler needs the blocks contiguous."""
     if z is None:
         z = np.sort(rng.integers(0, k, N))
     z = np.asarray(z)
-    pv = np.asarray(p, dtype=np.float64)
-    pv = pv * np.ones(k) if pv.size == 1 else pv
-    if pv.shape != (k,):
-        raise ValueError("Optional parameter p is neither a scalar nor a vector of length k.")
-    if q is None:
-        q = 0.3 / k
-    M = np.asarray(q, dtype=np.float64)
-    M = M * np.ones((k, k)) if M.size == 1 else M.copy()
-    if M.shape != (k, k):
-        raise ValueError("Optional parameter q is neither a scalar nor a matrix of size k x k.")
-    M.flat[::k + 1] = pv
+    if M is None:
+        pv = np.asarray(p, dtype=np.float64)
+        pv = pv * np.ones(k) if pv.size == 1 else pv
+        if pv.shape != (k,):
+            raise ValueError("Optional parameter p is neither a scalar nor a vector of length k.")
+        if q is None:
+            q = 0.3 / k
+        M = np.asarray(q, dtype=np.float64)
+        M = M * np.ones((k, k)) if M.size == 1 else M.copy()
+        if M.shape != (k, k):
+            raise ValueError("Optional parameter q is neither a scalar nor a matrix of size k x k.")
+        M.flat[::k + 1] = pv
+    else:
+        M = np.array(M, dtype=np.float64)
+        if M.shape != (k, k):
+            raise ValueError("M must be a matrix of size k x k.")
     if (M < 0).any() or (M > 1).any():
         raise ValueError("Probabilities should be in [0, 1].")
-    if np.any(np.diff(z) < 0):
+    if z.shape != (N,) or (N and (z.min() < 0 or z.max() >= k)):
+        raise ValueError("z must hold N block indices in [0, k).")
+    if sorted_z and np.any(np.diff(z) < 0):
         raise ValueError("z must be sorted (blocks contiguous) for the vectorised sampler")
     return z, M
 
 
-def _sbm_draw(rng, N, k, z, M):
-    """One draw of the SBM adjacency (canonical CSR) for blocks z and probabilities M."""
+def _sbm_draw(rng, N, k, z, M, directed=False, self_loops=False):
+    """One draw of the SBM adjacency (canonical CSR) for blocks z and probabilities M.
+
+    The pair spaces and their decoders are those of the device sampler (graphs/random_graphs.py):
+    undirected block pairs b <= a, every ordered pair when directed."""
+    from .random_graphs import decode_pairs, pair_space
     start = np.searchsorted(z, np.arange(k), side="left")
     size = np.searchsorted(z, np.arange(k), side="right") - start
 
@@ -843,21 +855,13 @@ def _sbm_draw(rng, N, k, z, M):
 
     rows, cols = [], []
     for a in range(k):
-        for b in range(a + 1):
-            if a == b:
-                n_pairs = int(size[a]) * (int(size[a]) - 1) // 2
-            else:
-                n_pairs = int(size[a]) * int(size[b])
+        for b in range(k if directed else a + 1):
+            kind, n_pairs, width = pair_space(int(size[a]), int(size[b]), a == b, directed,
+                                              self_loops)
             if n_pairs == 0 or M[a, b] == 0:
                 continue
             idx = distinct(n_pairs, int(rng.binomial(n_pairs, M[a, b])))
-            if a == b:            # index -> (i > j) of the strict lower triangle
-                i = np.floor((1 + np.sqrt(1 + 8 * idx.astype(np.float64))) / 2).astype(np.int64)
-                i -= (i * (i - 1) // 2 > idx)
-                i += ((i + 1) * i // 2 <= idx)
-                j = idx - i * (i - 1) // 2
-            else:
-                i, j = idx // int(size[b]), idx % int(size[b])
+            i, j = decode_pairs(kind, idx, width)
             rows.append(start[a] + i)
             cols.append(start[b] + j)
     if rows:
@@ -865,30 +869,61 @@ def _sbm_draw(rng, N, k, z, M):
         c = np.concatenate(cols)
     else:
         r = c = np.zeros(0, dtype=np.int64)
-    W = sparse.coo_matrix((np.ones(2 * r.size), (np.concatenate([r, c]), np.concatenate([c, r]))),
-                          shape=(N, N)).tocsr()
+    if not directed:              # both orientations, a loop once
+        off = r != c
+        r, c = np.concatenate([r, c[off]]), np.concatenate([c, r[off]])
+    W = sparse.coo_matrix((np.ones(r.size), (r, c)), shape=(N, N)).tocsr()
     W.sort_indices()
     return W
 
 
 class StochasticBlockModel(Graph):
-    r"""Stochastic block model graph (undirected, no self-loops); see :func:`sbm_adjacency`.
+    r"""Stochastic block model graph (pygsp/graphs/stochasticblockmodel.py:61-165).
 
-    ``connected=True`` draws z once and then resamples W from the same generator until the
-    graph is connected, at most ``n_try`` times (None: forever), as
-    stochasticblockmodel.py:125-157 does; it raises the reference's ``ValueError`` after
-    ``n_try`` failures.  With ``connected=False`` the graph is :func:`sbm_adjacency`'s.
+    Edge (i, j) is present with probability ``M[z_i, z_j]``, unit weights; ``M`` is given or
+    built from ``p`` (diagonal) and ``q`` (off the diagonal).  An undirected graph reads the
+    lower triangle of ``M``, as the reference does for a sorted ``z``; ``directed`` draws every
+    ordered pair, ``self_loops`` the pairs (i, i) too.
+
+    ``backend='host'`` (the default) is :func:`sbm_adjacency`'s sampler: block edge counts from
+    the binomial law, then that many distinct pairs; it needs ``z`` sorted.  ``backend='device'``
+    walks every block pair's Bernoulli process on the GPU from a Philox key
+    (graphs/random_graphs.py); ``z`` need not be sorted there, but an undirected graph with an
+    asymmetric ``M`` and an unsorted ``z`` raises ``ValueError``, since a pair's probability
+    would then depend on the vertex numbering.  Both draw ``z`` from
+    ``np.random.default_rng(seed)``; the device draws one key per trial from it after ``z``.
+
+    ``connected=True`` draws z once and then resamples W until the graph is connected, at most
+    ``n_try`` times (None: forever), as stochasticblockmodel.py:125-157 does; it raises the
+    reference's ``ValueError`` after ``n_try`` failures.
     """
 
     def __init__(self, N=1024, k=5, z=None, p=0.7, q=None, seed=None, connected=False,
-                 n_try=10, **kwargs):
+                 n_try=10, *, M=None, directed=False, self_loops=False, backend="host",
+                 **kwargs):
+        if backend not in ("host", "device"):
+            raise ValueError("Unknown backend {}.".format(backend))
         self.k, self.p, self.q, self.seed = k, p, q, seed
+        self.directed, self.self_loops = directed, self_loops
         self.connected, self.n_try = connected, n_try
         rng = np.random.default_rng(seed)
-        self.z, M = _sbm_blocks(rng, N, k, z, p, q)
+        self.z, self.M = _sbm_blocks(rng, N, k, z, p, q, M, sorted_z=backend == "host")
+        if (backend == "device" and not directed and np.any(np.diff(self.z) < 0)
+                and not np.array_equal(self.M, self.M.T)):
+            raise ValueError("An undirected graph with an asymmetric M needs z sorted: the "
+                             "probability of a pair would depend on the vertex numbering.")
+
+        def draw():
+            if backend == "host":
+                return _sbm_draw(rng, N, k, self.z, self.M, directed, self_loops)
+            from .random_graphs import sbm_device
+            return sbm_device(N, k, self.z, self.M, directed, self_loops,
+                              int(rng.integers(2 ** 63)), kwargs.get("dtype"),
+                              kwargs.get("device"))
+
         W = None
         while n_try is None or n_try > 0:
-            W = _sbm_draw(rng, N, k, self.z, M)
+            W = draw()
             if not connected or Graph(W, dtype=kwargs.get("dtype"),
                                       device=kwargs.get("device")).is_connected():
                 break
@@ -898,7 +933,17 @@ class StochasticBlockModel(Graph):
             raise ValueError("The graph could not be connected after {} trials. Increase the "
                              "connection probability or the number of trials.".format(self.n_try))
         if W is None:
-            W = _sbm_draw(rng, N, k, self.z, M)
+            W = draw()
         self.info = {"node_com": self.z, "comm_sizes": np.bincount(self.z, minlength=k),
                      "world_rad": np.sqrt(N)}
         super().__init__(W, **kwargs)
+
+    def _get_extra_repr(self):
+        attrs = {"k": self.k}
+        if type(self.p) is float:
+            attrs["p"] = f"{self.p:.2f}"
+        if type(self.q) is float:
+            attrs["q"] = f"{self.q:.2f}"
+        attrs.update({"directed": self.directed, "self_loops": self.self_loops,
+                      "connected": self.connected, "seed": self.seed})
+        return attrs
