@@ -181,6 +181,31 @@ __global__ void coo_keys_kernel(int64_t nnz, const int32_t* __restrict__ rows,
   keys[k] = (uint64_t(uint32_t(r)) << 32) | uint32_t(c);
 }
 
+// head[k] = 1 where the sorted keys start a new (row, col)
+__global__ void run_heads_kernel(int64_t nnz, const uint64_t* __restrict__ keys, int32_t* head) {
+  const int64_t k = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (k < nnz) head[k] = (k == 0 || keys[k] != keys[k - 1]) ? 1 : 0;
+}
+
+// One thread per run of equal keys adds the run's values one after the other, starting from the
+// first: the arithmetic of scipy's sum_duplicates.  The radix sort is stable, so the run is in
+// emission order.  rank[k] is the inclusive scan of the head flags; the last thread stores the
+// number of runs.
+template <typename T>
+__global__ void run_sum_kernel(int64_t nnz, const uint64_t* __restrict__ keys,
+                               const T* __restrict__ vals, const int32_t* __restrict__ rank,
+                               uint64_t* ukeys, T* data, int* n_unique) {
+  const int64_t k = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (k >= nnz) return;
+  if (k == nnz - 1) *n_unique = rank[k];
+  const uint64_t key = keys[k];
+  if (k > 0 && keys[k - 1] == key) return;
+  T acc = vals[k];
+  for (int64_t j = k + 1; j < nnz && keys[j] == key; ++j) acc += vals[j];
+  ukeys[rank[k] - 1] = key;
+  data[rank[k] - 1] = acc;
+}
+
 __global__ void coo_unpack_kernel(int64_t nuniq, const uint64_t* __restrict__ keys,
                                   int32_t* indices, int32_t* indptr) {
   const int64_t k = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -189,9 +214,9 @@ __global__ void coo_unpack_kernel(int64_t nuniq, const uint64_t* __restrict__ ke
   atomicAdd(indptr + int32_t(keys[k] >> 32) + 1, 1);
 }
 
-// Sorts by (row, col), sums duplicates; writes indptr and the first *n_unique_out
-// entries of indices / data (both sized nnz by the caller).  Synchronises the stream
-// once to return the number of distinct entries.
+// Sorts by (row, col), sums duplicates sequentially in emission order; writes indptr and
+// the first *n_unique_out entries of indices / data (both sized nnz by the caller).
+// Synchronises the stream once to return the number of distinct entries.
 template <typename T>
 static int coo_to_csr(int64_t n, int64_t nnz, const int32_t* rows, const int32_t* cols,
                       const T* vals, int32_t* indptr, int32_t* indices, T* data,
@@ -201,11 +226,13 @@ static int coo_to_csr(int64_t n, int64_t nnz, const int32_t* rows, const int32_t
   if (nnz == 0) return GSP_OK;
   Scratch<uint64_t> k0(st), k1(st), ku(st);
   Scratch<T> v1(st);
+  Scratch<int32_t> rank(st);
   Scratch<int> scal(st);     // [0] bad indices, [1] number of unique keys
   GSP_CUDA(k0.alloc(nnz));
   GSP_CUDA(k1.alloc(nnz));
   GSP_CUDA(ku.alloc(nnz));
   GSP_CUDA(v1.alloc(nnz));
+  GSP_CUDA(rank.alloc(nnz));
   GSP_CUDA(scal.alloc(2));
   GSP_CUDA(cudaMemsetAsync(scal.get(), 0, 2 * sizeof(int), st));
   coo_keys_kernel<<<(int)ceil_div(nnz, 256), 256, 0, st>>>(nnz, rows, cols, n, k0.get(),
@@ -218,11 +245,16 @@ static int coo_to_csr(int64_t n, int64_t nnz, const int32_t* rows, const int32_t
                                            (int)nnz, 0, bits, st);
   });
   if (rc != GSP_OK) return rc;
-  rc = cub_temp("cub::DeviceReduce::ReduceByKey", st, [&](void* tmp, size_t& bytes) {
-    return cub::DeviceReduce::ReduceByKey(tmp, bytes, k1.get(), ku.get(), v1.get(), data,
-                                          scal.get() + 1, cub::Sum(), (int)nnz, st);
+  const int blocks = (int)ceil_div(nnz, 256);
+  run_heads_kernel<<<blocks, 256, 0, st>>>(nnz, k1.get(), rank.get());
+  GSP_LAUNCH_CHECK("coo_run_heads");
+  rc = cub_temp("cub::DeviceScan::InclusiveSum", st, [&](void* tmp, size_t& bytes) {
+    return cub::DeviceScan::InclusiveSum(tmp, bytes, rank.get(), rank.get(), (int)nnz, st);
   });
   if (rc != GSP_OK) return rc;
+  run_sum_kernel<T><<<blocks, 256, 0, st>>>(nnz, k1.get(), v1.get(), rank.get(), ku.get(), data,
+                                            scal.get() + 1);
+  GSP_LAUNCH_CHECK("coo_run_sum");
   int host[2] = {0, 0};
   GSP_CUDA(cudaMemcpyAsync(host, scal.get(), sizeof(host), cudaMemcpyDeviceToHost, st));
   GSP_CUDA(cudaStreamSynchronize(st));

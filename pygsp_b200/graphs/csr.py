@@ -25,6 +25,16 @@ def row_ids(indptr):
     return torch.repeat_interleave(torch.arange(indptr.numel() - 1, device=indptr.device), counts)
 
 
+def index32(ids, n, device):
+    """Contiguous int32 copy of integer ids on ``device``.  int64 ids outside [0, n) become -1,
+    which the range checks of the kernels refuse; a plain cast would wrap 2^32 + k onto k."""
+    import torch
+    ids = ids.to(device)
+    if ids.dtype == torch.int64:
+        ids = torch.where((ids >= 0) & (ids < n), ids, -1)
+    return ids.to(torch.int32).contiguous()
+
+
 class DeviceCSR:
     def __init__(self, indptr, indices, data, shape):
         self.indptr = indptr
@@ -127,9 +137,13 @@ class DeviceCSR:
     @classmethod
     def from_coo(cls, rows, cols, vals, shape):
         """Canonical CSR of COO triplets in HBM: what ``sparse.csr_matrix(coo)`` does at
-        graph.py:109 -- sort by (row, col), sum duplicates in emission order -- on the device
-        (``gsp_coo_to_csr_*``).  Integer rows / cols, float32 or float64 vals; the result lives
-        on vals' device.  ``ValueError`` for 2^31 triplets or more, before anything is touched."""
+        graph.py:109 -- sort by (row, col), sum duplicates -- on the device
+        (``gsp_coo_to_csr_*``).  The values of one (row, col) are added one after the other in
+        the order they are given, in the value type, starting from the first (the arithmetic of
+        a sequential ``sum_duplicates``), so the result is reproducible bit for bit.  Integer
+        rows / cols, float32 or float64 vals; the result lives on vals' device.  An index
+        outside [0, n) raises ``NativeError``, int64 ones included (they are not cast to int32
+        first).  ``ValueError`` for 2^31 triplets or more, before anything is touched."""
         nnz = int(vals.numel())
         if nnz >= 2 ** 31:
             raise ValueError("The result would have {} entries; at most 2^31 - 1 are "
@@ -143,7 +157,7 @@ class DeviceCSR:
         uniq = ctypes.c_int64(0)
         with torch.cuda.device(dev):
             nat.call("gsp_coo_to_csr_" + nat.suffix(vals.dtype), nat.i64(n), nat.i64(nnz),
-                     rows.to(dev, torch.int32).contiguous(), cols.to(dev, torch.int32).contiguous(),
+                     index32(rows, n, dev), index32(cols, int(shape[1]), dev),
                      vals.contiguous(), indptr, indices, data, ctypes.byref(uniq),
                      nat.stream_ptr(dev))
         m = int(uniq.value)

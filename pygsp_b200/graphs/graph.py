@@ -22,7 +22,7 @@ from scipy import sparse
 from .. import _native as nat
 from .. import utils
 from .connectivity import ConnectivityMixIn
-from .csr import DeviceCSR
+from .csr import DeviceCSR, index32
 from .difference import DifferenceMixIn
 from .fourier import FourierMixIn
 from .layout import LayoutMixIn
@@ -79,7 +79,7 @@ class Graph(FourierMixIn, DifferenceMixIn, ConnectivityMixIn, LayoutMixIn):
         if W.data.dtype != self.dtype:
             W = DeviceCSR(W.indptr, W.indices, W.data.to(self.dtype), W.shape)
         W = DeviceCSR(W.indptr.to(self.device, torch.int32).contiguous(),
-                      W.indices.to(self.device, torch.int32).contiguous(),
+                      index32(W.indices, W.shape[1], self.device),
                       W.data.to(self.device).contiguous(), W.shape)
         self.n_vertices = W.shape[0]
 
@@ -130,10 +130,11 @@ class Graph(FourierMixIn, DifferenceMixIn, ConnectivityMixIn, LayoutMixIn):
 
     @classmethod
     def from_coo(cls, rows, cols, vals, n_vertices, lap_type="combinatorial", **kwargs):
-        """Graph from COO triplets already in HBM (int32 rows / cols, float values).
+        """Graph from COO triplets already in HBM (integer rows / cols, float values).
 
         What ``sparse.csr_matrix(coo)`` does at graph.py:109 -- sort by (row, col), sum
-        duplicates -- runs on the device (:meth:`DeviceCSR.from_coo`); no host matrix exists.
+        duplicates in the order given -- runs on the device (:meth:`DeviceCSR.from_coo`); no
+        host matrix exists.  An index outside [0, n_vertices) raises ``NativeError``.
         """
         torch = nat.require_cuda()
         dt = _torch_dtype(torch, kwargs.get("dtype", vals.dtype if vals.dtype in
