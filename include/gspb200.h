@@ -560,6 +560,26 @@ int gsp_cheby_op_dist_f64(const gsp_dist_plan* plan_host, const gsp_tile_plan* t
                           double lmax, const double* coeffs_host, int nscales, int m, const double* x,
                           int64_t nsig, double* r, int clenshaw, uint64_t* seq_host, void* stream);
 
+/* gsp_cheby_op_dist_phases_*: the same call cut into its m + 1 phases; enqueues phases
+ * [phase_begin, phase_end) only (gsp_cheby_op_dist_* is the range [0, m + 1)).  Each phase
+ * first waits, then pushes, so that several ranks can share one device and one stream when the
+ * caller runs phase j of every rank before phase j + 1 of any (base = *seq_host as passed in):
+ *   phase 0      entry barrier: publishes base+1, waits for nothing
+ *   phase 1      waits for base+1, brings in x (gather by perm, or copy), publishes base+2
+ *   phase 1 + s  recurrence step s = 1 .. m-1 (forward or Clenshaw): waits for base+1+s and
+ *                publishes base+2+s, except the last step, which publishes nothing
+ * The blocks a phase reads and writes depend on the phase alone.  *seq_host advances by m + 2
+ * only when phase_end == m + 1.  A forward-form range that is not the whole call refuses
+ * plan->perm (its accumulators are call-local then) with an error, before any launch. */
+int gsp_cheby_op_dist_phases_f32(const gsp_dist_plan* plan_host, const gsp_tile_plan* tile_host,
+                                 double lmax, const double* coeffs_host, int nscales, int m,
+                                 const float* x, int64_t nsig, float* r, int clenshaw,
+                                 uint64_t* seq_host, int phase_begin, int phase_end, void* stream);
+int gsp_cheby_op_dist_phases_f64(const gsp_dist_plan* plan_host, const gsp_tile_plan* tile_host,
+                                 double lmax, const double* coeffs_host, int nscales, int m,
+                                 const double* x, int64_t nsig, double* r, int clenshaw,
+                                 uint64_t* seq_host, int phase_begin, int phase_end, void* stream);
+
 /* ------------------------------------------------------ on-device graph construction ---
  * gsp_grid2d_*: adjacency of pygsp/graphs/grid2d.py:40-89 (n1 x n2 grid, 4 neighbours, unit
  *     weights, row-major numbering) as canonical CSR; count writes indptr (n1*n2 + 1).

@@ -109,18 +109,21 @@ struct StepTrace {
 template <typename T>
 int cheby_op_dist(const gsp_dist_plan* p, const gsp_tile_plan* tile, double lmax, const double* c,
                   int nscales, int m, const T* x, int64_t nsig64, T* r, int clenshaw,
-                  uint64_t* seq, void* stream) {
+                  uint64_t* seq, int phase_begin, int phase_end, void* stream) {
   GSP_REQUIRE(p && seq && r, "null argument");
   GSP_REQUIRE(m >= 2, "The coefficients have an invalid shape");        // approximations.py:83-84
   GSP_REQUIRE(nscales >= 1 && nscales <= 16, "1..16 filters per call");
   GSP_REQUIRE(lmax > 0 && lmax == lmax, "lmax must be positive");
   GSP_REQUIRE(nsig64 >= 1 && nsig64 <= (1 << 20), "nsig out of range");
+  const int K = m - 1;
+  // phases: 0 entry barrier, 1 input block and halo of T_0, 1 + s recurrence step s = 1 .. K
+  GSP_REQUIRE(0 <= phase_begin && phase_begin <= phase_end && phase_end <= K + 2,
+              "phase range out of bounds");
+  const bool whole = phase_begin == 0 && phase_end == K + 2;
+  auto in = [&](int phase) { return phase >= phase_begin && phase < phase_end; };
   const int nsig = int(nsig64);
   const int64_t n = p->n_local;
-  const int K = m - 1;
   cudaStream_t st = as_stream(stream);
-  const uint64_t base = *seq;
-  *seq = base + uint64_t(m) + 2;
   T* buf[3] = {static_cast<T*>(p->buf[0]), static_cast<T*>(p->buf[1]), static_cast<T*>(p->buf[2])};
   // a step fuses the exchange when this holds and the tiled kernel takes it (dist_step)
   const bool fusable =
@@ -128,25 +131,34 @@ int cheby_op_dist(const gsp_dist_plan* p, const gsp_tile_plan* tile, double lmax
       p->n_neighbors <= 32 &&
       std::max(p->n_push_rows, p->n_boundary_rows) <= (n / tile->rows_per_tile) * tile->rows_per_tile;
   if (clenshaw && (nscales != 1 || K < 2 || !buf[2])) clenshaw = 0;
+  const int64_t* perm = p->perm;      // local row i is row perm[i] of the caller's block
+  // the forward form keeps its accumulators in call-local scratch when it permutes rows
+  GSP_REQUIRE(whole || clenshaw || !perm, "a phased forward call takes no row permutation");
+  const uint64_t base = *seq;
+  if (phase_end == K + 2) *seq = base + uint64_t(m) + 2;
 
   StepTrace trace(st);
   trace.mark();
-  // entry barrier, input block, halo of T_0
-  int rc = DistTraits<T>::push(p, 0, 0, base + 1, nsig, stream);
-  if (rc != GSP_OK) return rc;
-  rc = gsp_halo_wait(p->flags, p->neighbor_ids, p->n_neighbors, base + 1, stream);
-  if (rc != GSP_OK) return rc;
-  const int64_t* perm = p->perm;      // local row i is row perm[i] of the caller's block
-  if (x && perm) {
-    rc = move_rows<T>(false, n, perm, x, nsig, buf[0], st);
+  int rc = GSP_OK;
+  if (in(0)) {        // entry barrier
+    rc = DistTraits<T>::push(p, 0, 0, base + 1, nsig, stream);
     if (rc != GSP_OK) return rc;
-  } else if (x && x != buf[0]) {
-    GSP_CUDA(cudaMemcpyAsync(buf[0], x, sizeof(T) * size_t(n) * nsig, cudaMemcpyDeviceToDevice, st));
   }
-  rc = DistTraits<T>::push(p, p->n_send, 0, base + 2, nsig, stream);
-  if (rc != GSP_OK) return rc;
-  trace.mark();
+  if (in(1)) {        // input block, halo of T_0
+    rc = gsp_halo_wait(p->flags, p->neighbor_ids, p->n_neighbors, base + 1, stream);
+    if (rc != GSP_OK) return rc;
+    if (x && perm) {
+      rc = move_rows<T>(false, n, perm, x, nsig, buf[0], st);
+      if (rc != GSP_OK) return rc;
+    } else if (x && x != buf[0]) {
+      GSP_CUDA(cudaMemcpyAsync(buf[0], x, sizeof(T) * size_t(n) * nsig, cudaMemcpyDeviceToDevice, st));
+    }
+    rc = DistTraits<T>::push(p, p->n_send, 0, base + 2, nsig, stream);
+    if (rc != GSP_OK) return rc;
+    trace.mark();
+  }
 
+  // Step s runs in phase 1 + s; the blocks it reads and writes depend on s alone.
   double ck[16], c0[16];
   Step<T> s{p->nnz, p->indptr, p->indices, static_cast<const T*>(p->data)};
   s.r_rows = n;
@@ -160,13 +172,15 @@ int cheby_op_dist(const gsp_dist_plan* p, const gsp_tile_plan* tile, double lmax
     s.r = local.get() ? local.get() : r;
     int cur = 0, old = 1;
     for (int k = 1; k <= K; ++k) {
-      forward_coefs(s, k, m, nscales, lmax, c, ck, c0);
-      s.x_cur = buf[cur];
-      s.x_old = s.first ? nullptr : buf[old];
-      s.x_new = buf[old];
-      rc = dist_step<T>(p, tile, fusable, s, old, base + 1 + k, base + 2 + k, k < K, stream);
-      if (rc != GSP_OK) return rc;
-      trace.mark();
+      if (in(1 + k)) {
+        forward_coefs(s, k, m, nscales, lmax, c, ck, c0);
+        s.x_cur = buf[cur];
+        s.x_old = s.first ? nullptr : buf[old];
+        s.x_new = buf[old];
+        rc = dist_step<T>(p, tile, fusable, s, old, base + 1 + k, base + 2 + k, k < K, stream);
+        if (rc != GSP_OK) return rc;
+        trace.mark();
+      }
       std::swap(cur, old);
     }
     if (local.get()) {
@@ -178,26 +192,30 @@ int cheby_op_dist(const gsp_dist_plan* p, const gsp_tile_plan* tile, double lmax
   }
   // Clenshaw, single filter (see cheby_clenshaw in cheby.cu): buf[0] keeps x (the source),
   // b_{K-1} -> buf[1], b_{K-2} -> buf[2], b_{K-3} -> buf[1], ...; the last step writes r.
-  clenshaw_coefs(s, K - 1, m, 1, lmax, c, ck);
-  s.x_cur = buf[0];
-  s.x_new = s.r = buf[1];
-  rc = dist_step<T>(p, tile, fusable, s, 1, base + 2, base + 3, true, stream);
-  if (rc != GSP_OK) return rc;
-  trace.mark();
-  s.r = buf[0];
+  if (in(2)) {
+    clenshaw_coefs(s, K - 1, m, 1, lmax, c, ck);
+    s.x_cur = buf[0];
+    s.x_new = s.r = buf[1];
+    rc = dist_step<T>(p, tile, fusable, s, 1, base + 2, base + 3, true, stream);
+    if (rc != GSP_OK) return rc;
+    trace.mark();
+  }
   int cur = 1, old = -1, step = 1;
   for (int k = K - 2; k >= 0; --k) {
     ++step;
     const bool last = k == 0;
-    clenshaw_coefs(s, k, m, 1, lmax, c, ck);
     const int dst = last ? -1 : (old >= 0 ? old : 2);
-    s.x_cur = buf[cur];
-    s.x_old = buf[old >= 0 ? old : cur];   // no b_{k+2} yet: any valid block, times gamma = 0
-    s.x_new = last ? r : buf[dst];
-    s.out_perm = last ? perm : nullptr;
-    rc = dist_step<T>(p, tile, fusable, s, dst, base + 1 + step, base + 2 + step, !last, stream);
-    if (rc != GSP_OK) return rc;
-    trace.mark();
+    if (in(1 + step)) {
+      clenshaw_coefs(s, k, m, 1, lmax, c, ck);
+      s.r = buf[0];
+      s.x_cur = buf[cur];
+      s.x_old = buf[old >= 0 ? old : cur];   // no b_{k+2} yet: any valid block, times gamma = 0
+      s.x_new = last ? r : buf[dst];
+      s.out_perm = last ? perm : nullptr;
+      rc = dist_step<T>(p, tile, fusable, s, dst, base + 1 + step, base + 2 + step, !last, stream);
+      if (rc != GSP_OK) return rc;
+      trace.mark();
+    }
     old = cur;
     cur = dst;
   }
@@ -207,16 +225,30 @@ int cheby_op_dist(const gsp_dist_plan* p, const gsp_tile_plan* tile, double lmax
 }  // namespace gsp
 
 extern "C" {
+int gsp_cheby_op_dist_phases_f32(const gsp_dist_plan* plan_host, const gsp_tile_plan* tile_host,
+                                 double lmax, const double* coeffs_host, int nscales, int m,
+                                 const float* x, int64_t nsig, float* r, int clenshaw,
+                                 uint64_t* seq_host, int phase_begin, int phase_end, void* stream) {
+  return gsp::cheby_op_dist<float>(plan_host, tile_host, lmax, coeffs_host, nscales, m, x, nsig, r,
+                                   clenshaw, seq_host, phase_begin, phase_end, stream);
+}
+int gsp_cheby_op_dist_phases_f64(const gsp_dist_plan* plan_host, const gsp_tile_plan* tile_host,
+                                 double lmax, const double* coeffs_host, int nscales, int m,
+                                 const double* x, int64_t nsig, double* r, int clenshaw,
+                                 uint64_t* seq_host, int phase_begin, int phase_end, void* stream) {
+  return gsp::cheby_op_dist<double>(plan_host, nullptr, lmax, coeffs_host, nscales, m, x, nsig, r,
+                                    clenshaw, seq_host, phase_begin, phase_end, stream);
+}
 int gsp_cheby_op_dist_f32(const gsp_dist_plan* plan_host, const gsp_tile_plan* tile_host,
                           double lmax, const double* coeffs_host, int nscales, int m, const float* x,
                           int64_t nsig, float* r, int clenshaw, uint64_t* seq_host, void* stream) {
-  return gsp::cheby_op_dist<float>(plan_host, tile_host, lmax, coeffs_host, nscales, m, x, nsig, r,
-                                   clenshaw, seq_host, stream);
+  return gsp_cheby_op_dist_phases_f32(plan_host, tile_host, lmax, coeffs_host, nscales, m, x, nsig,
+                                      r, clenshaw, seq_host, 0, m + 1, stream);
 }
 int gsp_cheby_op_dist_f64(const gsp_dist_plan* plan_host, const gsp_tile_plan* tile_host,
                           double lmax, const double* coeffs_host, int nscales, int m, const double* x,
                           int64_t nsig, double* r, int clenshaw, uint64_t* seq_host, void* stream) {
-  return gsp::cheby_op_dist<double>(plan_host, nullptr, lmax, coeffs_host, nscales, m, x, nsig, r,
-                                    clenshaw, seq_host, stream);
+  return gsp_cheby_op_dist_phases_f64(plan_host, tile_host, lmax, coeffs_host, nscales, m, x, nsig,
+                                      r, clenshaw, seq_host, 0, m + 1, stream);
 }
 }

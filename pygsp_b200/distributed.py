@@ -526,6 +526,86 @@ class PartitionedCheby:
         return r
 
 
+def _neighbors(plan):
+    """The ranks this rank exchanges halo rows with, ascending."""
+    return [q for q in range(plan.parts)
+            if q != plan.rank and (plan.send_counts[q] > 0 or plan.recv_counts[q] > 0)]
+
+
+class PeerTables:
+    """The device tables of one rank's ``gsp_dist_plan`` and the plan itself (``dist_plan``).
+
+    Pure host computation from the rank's ``HaloPlan`` and what every rank publishes about its
+    window: ``infos[q] = (n_local, recv_counts, buf_bytes)`` of rank q, and ``bases[q]``, the
+    device address at which THIS rank sees rank q's window (its own for q == rank; None for
+    ranks that are not neighbours).  A window is ``buf0 | buf1 | buf2 | flags[P] (uint64) |
+    push counter (uint32) | fused counter (uint64, at +8)``.  ``indptr`` / ``indices`` /
+    ``data`` / ``send_idx`` are the rank's device tensors.  The tables live as long as this
+    object; ``dist_plan`` points into them.
+    """
+
+    def __init__(self, plan, infos, bases, indptr, indices, data, send_idx, n_bufs=3):
+        import torch
+        p = plan
+        dev = send_idx.device
+        self.neighbors = _neighbors(p)
+        # destination row of every packed row: the slot the neighbour reserved for it
+        dst_peer, dst_row = [], []
+        for q in range(p.parts):
+            cnt = int(p.send_counts[q])
+            if cnt == 0:
+                continue
+            n_local_q, recv_q = infos[q][0], infos[q][1]
+            first = n_local_q + int(sum(recv_q[:p.rank]))     # q's halo slots are owner-ordered
+            dst_peer.append(np.full(cnt, q, dtype=np.int32))
+            dst_row.append(first + np.arange(cnt, dtype=np.int64))
+        cat = lambda parts, dt: torch.from_numpy(
+            np.concatenate(parts) if parts else np.zeros(0, dtype=dt)).to(dev)
+        self.dst_peer = cat(dst_peer, np.int32)
+        self.dst_row = cat(dst_row, np.int64)
+        self.src_row = send_idx
+        base_tab = np.zeros((n_bufs, p.parts), dtype=np.int64)
+        for q in self.neighbors:
+            for b in range(n_bufs):
+                base_tab[b, q] = bases[q] + b * infos[q][2]
+        self.peer_base = torch.from_numpy(base_tab).to(dev)                  # pointers as int64
+        flag_tab = np.array([bases[q] + n_bufs * infos[q][2] + 8 * p.rank
+                             for q in self.neighbors], dtype=np.int64)
+        self.peer_flags = torch.from_numpy(flag_tab).to(dev)
+        self.neighbor_ids = torch.from_numpy(np.asarray(self.neighbors, dtype=np.int32)).to(dev)
+        # the same send list as a CSR over the local rows, for the fused epilogue push
+        src = p.send_idx
+        order = np.argsort(src, kind="stable")
+        self.n_push_rows = int(src.max()) + 1 if src.size else 0
+        ptr = np.zeros(self.n_push_rows + 1, dtype=np.int64)
+        np.add.at(ptr, src + 1, 1)
+        self.push_ptr = torch.from_numpy(np.cumsum(ptr).astype(np.int32)).to(dev)
+        self.push_peer = self.dst_peer[torch.from_numpy(order).to(dev)].contiguous()
+        self.push_row = self.dst_row[torch.from_numpy(order).to(dev)].contiguous()
+        own, buf_bytes = bases[p.rank], infos[p.rank][2]
+        flags_ptr = own + n_bufs * buf_bytes
+        counter_ptr = flags_ptr + 8 * p.parts
+        d = nat.DistPlan()
+        d.n_local, d.n_halo, d.nnz = p.n_local, p.n_halo, p.nnz
+        d.indptr, d.indices, d.data = indptr.data_ptr(), indices.data_ptr(), data.data_ptr()
+        for b in range(n_bufs):
+            d.buf[b] = own + b * buf_bytes
+            d.peer_base[b] = self.peer_base[b].data_ptr()
+        d.peer_flags = self.peer_flags.data_ptr()
+        d.flags = flags_ptr
+        d.neighbor_ids = self.neighbor_ids.data_ptr()
+        d.n_neighbors = len(self.neighbors)
+        d.push_counter, d.fused_counter = counter_ptr, counter_ptr + 8
+        d.n_send = int(self.src_row.numel())
+        d.src_row, d.dst_peer, d.dst_row = (self.src_row.data_ptr(), self.dst_peer.data_ptr(),
+                                            self.dst_row.data_ptr())
+        d.n_push_rows = self.n_push_rows
+        d.push_ptr, d.push_peer, d.push_row = (self.push_ptr.data_ptr(), self.push_peer.data_ptr(),
+                                               self.push_row.data_ptr())
+        d.n_boundary_rows = p.n_true_boundary
+        self.dist_plan = d
+
+
 class PeerWindow:
     """State buffers + flags of one rank for one signal width, IPC-mapped by its neighbours.
 
@@ -553,76 +633,23 @@ class PeerWindow:
         self.base = int(ptr.value)
         self.bufs = [_wrap(self.base + b * self.buf_bytes, (ext, nsig), op.dtype, op.device)
                      for b in range(self.n_bufs)]
-        self.flags_ptr = self.base + flag_off
-        self.counter_ptr = self.flags_ptr + 8 * p.parts
         # everybody learns everybody's handle, block size and halo layout
         info = [None] * p.parts
         dist.all_gather_object(info, (bytes(handle), int(p.n_local), p.recv_counts.tolist(),
                                       int(self.buf_bytes)), group=op.group)
-        self.neighbors = [q for q in range(p.parts)
-                          if q != p.rank and (p.send_counts[q] > 0 or p.recv_counts[q] > 0)]
         self.opened = {}
-        for q in self.neighbors:
+        for q in _neighbors(p):
             qptr = ctypes.c_void_p()
             hq = (ctypes.c_ubyte * 64).from_buffer_copy(info[q][0])
             with torch.cuda.device(op.device):
                 nat.call("gsp_ipc_open", hq, ctypes.byref(qptr))
             self.opened[q] = int(qptr.value)
-        dev = op.device
-        # destination row of every packed row: the slot the neighbour reserved for it
-        dst_peer, dst_row = [], []
-        for q in range(p.parts):
-            cnt = int(p.send_counts[q])
-            if cnt == 0:
-                continue
-            n_local_q, recv_q = info[q][1], info[q][2]
-            first = n_local_q + int(sum(recv_q[:p.rank]))     # q's halo slots are owner-ordered
-            dst_peer.append(np.full(cnt, q, dtype=np.int32))
-            dst_row.append(first + np.arange(cnt, dtype=np.int64))
-        cat = lambda parts, dt: torch.from_numpy(
-            np.concatenate(parts) if parts else np.zeros(0, dtype=dt)).to(dev)
-        self.dst_peer = cat(dst_peer, np.int32)
-        self.dst_row = cat(dst_row, np.int64)
+        bases = [self.base if q == p.rank else self.opened.get(q) for q in range(p.parts)]
+        self.tables = PeerTables(p, [i[1:] for i in info], bases, op.indptr, op.indices, op.data,
+                                 op.send_idx, self.n_bufs)
         self.src_row = op.send_idx
-        base_tab = np.zeros((self.n_bufs, p.parts), dtype=np.int64)
-        for q, qbase in self.opened.items():
-            for b in range(self.n_bufs):
-                base_tab[b, q] = qbase + b * info[q][3]
-        self.peer_base = torch.from_numpy(base_tab).to(dev)                  # pointers as int64
-        flag_tab = np.array([self.opened[q] + self.n_bufs * info[q][3] + 8 * p.rank
-                             for q in self.neighbors], dtype=np.int64)
-        self.peer_flags = torch.from_numpy(flag_tab).to(dev)
-        self.neighbor_ids = torch.from_numpy(np.asarray(self.neighbors, dtype=np.int32)).to(dev)
-        # the same send list as a CSR over the local rows, for the fused epilogue push
-        src = p.send_idx
-        order = np.argsort(src, kind="stable")
-        self.n_push_rows = int(src.max()) + 1 if src.size else 0
-        ptr = np.zeros(self.n_push_rows + 1, dtype=np.int64)
-        np.add.at(ptr, src + 1, 1)
-        self.push_ptr = torch.from_numpy(np.cumsum(ptr).astype(np.int32)).to(dev)
-        self.push_peer = self.dst_peer[torch.from_numpy(order).to(dev)].contiguous()
-        self.push_row = self.dst_row[torch.from_numpy(order).to(dev)].contiguous()
-        self.fused_counter_ptr = self.counter_ptr + 8
-        d = nat.DistPlan()
-        d.n_local, d.n_halo, d.nnz = p.n_local, p.n_halo, p.nnz
-        d.indptr, d.indices, d.data = op.indptr.data_ptr(), op.indices.data_ptr(), op.data.data_ptr()
-        for b in range(self.n_bufs):
-            d.buf[b] = self.bufs[b].data_ptr()
-            d.peer_base[b] = self.peer_base[b].data_ptr()
-        d.peer_flags = self.peer_flags.data_ptr()
-        d.flags = self.flags_ptr
-        d.neighbor_ids = self.neighbor_ids.data_ptr()
-        d.n_neighbors = len(self.neighbors)
-        d.push_counter, d.fused_counter = self.counter_ptr, self.fused_counter_ptr
-        d.n_send = int(self.src_row.numel())
-        d.src_row, d.dst_peer, d.dst_row = (self.src_row.data_ptr(), self.dst_peer.data_ptr(),
-                                            self.dst_row.data_ptr())
-        d.n_push_rows = self.n_push_rows
-        d.push_ptr, d.push_peer, d.push_row = (self.push_ptr.data_ptr(), self.push_peer.data_ptr(),
-                                               self.push_row.data_ptr())
-        d.n_boundary_rows = p.n_true_boundary
-        self.dist_plan = d
-        torch.cuda.synchronize(dev)
+        self.dist_plan = self.tables.dist_plan
+        torch.cuda.synchronize(op.device)
         if p.parts > 1:
             dist.barrier(group=op.group)
 
