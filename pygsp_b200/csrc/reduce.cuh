@@ -1,10 +1,13 @@
 // Fixed-order reductions: the summation order behind every bit-reproducible device solver.
 //
 // Column sums over rows (csrc/block.cu, csrc/krylov.cu, csrc/moments.cu) are two-level.
-// row_parts splits the n rows into at most kMaxParts parts of >= 1024 rows, a function of n
-// alone; CTA p sums part p with column_part (lane = column, warp w takes rows w, w + 8, ... in
-// order, the warp sums are added in warp order) and sum_parts adds the partials in p order.  So a
-// column's bits do not depend on the other columns, on how many there are or on the device.
+// row_parts splits the n rows into min(ceil(n / 1024), kMaxParts) parts of ceil(n / parts) rows
+// (the last may be shorter), a function of n alone: parts are at most 1024 rows up to
+// kMaxParts * 1024 rows and longer only past it (n = 1025 gives two parts of 513 rows,
+// n = 263 * 1024 + 1 gives 264 parts of 1021); CTA p sums part p with column_part (lane =
+// column, warp w takes rows w, w + 8, ... in order, the warp sums are added in warp order) and
+// sum_parts adds the partials in p order.  So a column's bits do not depend on the other
+// columns, on how many there are or on the device.
 // csrc/cg.cu forms its own per-CTA partials and adds them with sum_parts.
 //
 // A FISTA pass (csrc/simplex.cu, csrc/tv.cu) is one launch of pass_blocks CTAs whose last CTA to

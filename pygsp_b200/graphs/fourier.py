@@ -371,9 +371,21 @@ def block_width(k, n):
 
 
 # ------------------------------------------------------------------ block kernels
+def _same_block(what, A, B):
+    """ValueError unless A and B are blocks of one dtype, on one device, with as many rows: the
+    kernels read both through A's element type and row count."""
+    if A.dtype != B.dtype:
+        raise ValueError("%s: dtypes differ (%s, %s)" % (what, A.dtype, B.dtype))
+    if A.device != B.device:
+        raise ValueError("%s: devices differ (%s, %s)" % (what, A.device, B.device))
+    if A.shape[0] != B.shape[0]:
+        raise ValueError("%s: row counts differ (%d, %d)" % (what, A.shape[0], B.shape[0]))
+
+
 def block_gram(A, B):
     """A^T B (float64 device tensor) for (n, ka) and (n, kb) device blocks of one dtype."""
     torch = nat.require_cuda()
+    _same_block("block_gram", A, B)
     A, B = A.contiguous(), B.contiguous()
     A2, B2 = A.reshape(A.shape[0], -1), B.reshape(B.shape[0], -1)
     C = torch.empty((A2.shape[1], B2.shape[1]), dtype=torch.float64, device=A.device)
@@ -389,6 +401,9 @@ def block_combine(A, Q):
     A = A.contiguous()
     Q = torch.as_tensor(Q, dtype=torch.float64, device=A.device).contiguous()
     Q2 = Q.reshape(Q.shape[0], -1)
+    if A.dim() != 2 or Q2.shape[0] != A.shape[1]:
+        raise ValueError("block_combine: Q has %d rows for a block of shape %s"
+                         % (Q2.shape[0], tuple(A.shape)))
     Y = torch.empty((A.shape[0], Q2.shape[1]), dtype=A.dtype, device=A.device)
     with torch.cuda.device(A.device):
         nat.call("gsp_block_combine_" + nat.suffix(A.dtype), nat.i64(A.shape[0]), A,
@@ -399,7 +414,15 @@ def block_combine(A, Q):
 def block_residual(X, LX, theta):
     """||LX[:, j] - theta[j] X[:, j]||^2 for every column (host float64 array)."""
     torch = nat.require_cuda()
-    th = torch.as_tensor(np.asarray(theta, dtype=np.float64), device=X.device)
+    _same_block("block_residual", X, LX)
+    if X.dim() != 2 or LX.shape != X.shape:
+        raise ValueError("block_residual: shapes %s and %s" % (tuple(X.shape), tuple(LX.shape)))
+    theta = np.asarray(theta, dtype=np.float64).ravel()
+    if theta.size != X.shape[1]:
+        raise ValueError("block_residual: %d values of theta for %d columns"
+                         % (theta.size, X.shape[1]))
+    X, LX = X.contiguous(), LX.contiguous()
+    th = torch.as_tensor(theta, device=X.device)
     out = torch.empty(X.shape[1], dtype=torch.float64, device=X.device)
     with torch.cuda.device(X.device):
         nat.call("gsp_block_residual_" + nat.suffix(X.dtype), nat.i64(X.shape[0]), X, LX, th,
