@@ -151,6 +151,43 @@ int gsp_cheby_step_halo_f32(int first, int64_t n_rows, int64_t nnz, const int32_
 GSPB200_DECLARE_CHEBY_API(f32, float)
 GSPB200_DECLARE_CHEBY_API(f64, double)
 
+/* Filter banks wider than 16 filters (csrc/cheby_bank.cu).
+ *
+ * gsp_cheby_op_basis_*: pygsp/filters/approximations.py:58-114 `cheby_op(G, c, signal)` for any
+ *   number of filters.  The m - 1 recurrence steps write T_k x into slot k of basis
+ *   ((m, n, nsig), caller-given; slot 0 stands for T_0 = x and is read only when x is slot 0
+ *   itself, otherwise it is not written), with no accumulator; then one combine pass forms
+ *   r_i = sum_k c_ik T_k x for every filter, reading the basis once and writing each output once.
+ *   coeffs is a DEVICE (nscales, m) row-major double matrix; r receives (nscales, n, ldr) with
+ *   ldr >= nsig (a column range of a wider block: row j of filter i at r + (i n + j) ldr).  The
+ *   combine forms fma(c_i1, T_1, (c_i0/2) T_0), then fma(c_ik, T_k, r) for increasing k, with the
+ *   coefficients cast to T as the fused step casts them, so r is the bits of gsp_cheby_op_* on
+ *   the same block.  Every step is one gsp_cheby_step_* (plan_host: the tiling for nscales = 0).
+ *   No allocation, no synchronisation.
+ * gsp_cheby_synthesis_wide_*: filter.py:313-322 (the synthesis of an Nf-feature signal, one
+ *   forward recurrence per feature) for any nsrc.  One mix pass over the nsrc source blocks
+ *   ((nsrc, n, nsig) in memory) forms the per-order sources u_k = sum_f c'_fk s_f (c'_f0 =
+ *   c_f0 / 2, the sum in increasing f) for up to 32 orders, one more pass per further 32; then
+ *   one Clenshaw recurrence b_k = u_k + 2 Lt b_{k+1} - b_{k+2} runs with the source block of
+ *   order k (m - 1 SpMMs).  coeffs is a DEVICE (nsrc, m) row-major double matrix; out is
+ *   (n, nsig); work holds (m + 2) n nsig elements; plan_host is the tiling for nscales = 1.
+ *   Same value as gsp_cheby_clenshaw_*, different rounding (the sources are summed per order
+ *   before they enter the recurrence).  No allocation, no synchronisation. */
+#define GSPB200_DECLARE_BANK_API(SUF, T)                                                          \
+  int gsp_cheby_op_basis_##SUF(int64_t n, int64_t nnz, const int32_t* indptr,                     \
+                               const int32_t* indices, const T* data, double lmax,                \
+                               const double* coeffs, int nscales, int m, const T* x,              \
+                               int64_t nsig, T* basis, T* r, int64_t ldr,                         \
+                               const gsp_tile_plan* plan_host, void* stream);                     \
+  int gsp_cheby_synthesis_wide_##SUF(int64_t n, int64_t nnz, const int32_t* indptr,               \
+                                     const int32_t* indices, const T* data, double lmax,          \
+                                     const double* coeffs, int nsrc, int m, const T* sources,     \
+                                     int64_t nsig, T* out, T* work,                               \
+                                     const gsp_tile_plan* plan_host, void* stream);
+
+GSPB200_DECLARE_BANK_API(f32, float)
+GSPB200_DECLARE_BANK_API(f64, double)
+
 /* Clenshaw filtering of ONE float32 source with the middle steps run two per launch.  A paired
  * launch forms b_k into a third work block and b_{k-1} over b_{k+2} while b_k, b_{k+1} and the
  * source are still in L2: five passes over a signal block per two steps instead of eight, and

@@ -15,6 +15,10 @@ from .. import utils
 
 _logger = utils.build_logger(__name__)
 PATCH_DEFAULT_DTYPE = None     # engine dtype for reference (scipy) graphs, see patch_pygsp()
+# filters whose coefficients the fused step takes by value; wider banks and syntheses of more
+# features go through the stored basis (cheby_bank_device) and the per-order sources
+# (cheby_synthesis_wide_device)
+WIDE_BANK = 16
 
 
 @utils.filterbank_handler
@@ -114,6 +118,93 @@ def cheby_op_device(L, lmax, c, x, out=None, work=None):
     return r
 
 
+def _free_device_bytes(device):
+    torch = nat.require_cuda()
+    free, _ = torch.cuda.mem_get_info(device)
+    return free + torch.cuda.memory_reserved(device) - torch.cuda.memory_allocated(device)
+
+
+def cheby_bank_device(L, lmax, c, x, max_columns=None):
+    """Any filter bank through a stored Chebyshev basis: x (N, nsig) tensor -> (Nf, N, nsig).
+
+    The recurrence writes T_k x (k < m) into a basis buffer with no accumulator, and one combine
+    pass forms every r_i = sum_k c_ik T_k x (csrc/cheby_bank.cu, ``gsp_cheby_op_basis_*``): the
+    basis is read once and each output written once, however many filters there are.  The result
+    is the bits of :func:`cheby_op_device` on the same bank.  The basis takes m N nsig elements;
+    when that does not fit in the device memory left once the output is allocated (or
+    ``max_columns`` is given) the columns are processed in chunks, with the same bits, since no
+    sum mixes columns."""
+    torch = nat.require_cuda()
+    c = np.ascontiguousarray(np.atleast_2d(np.asarray(c, dtype=np.float64)))
+    nf, m = c.shape
+    if m < 2:
+        raise TypeError("The coefficients have an invalid shape")
+    n, nsig = x.shape
+    out = torch.empty((nf, n, nsig), dtype=L.dtype, device=L.device)
+    if nsig == 0 or n == 0:
+        return out
+    item = x.element_size()
+    per_column = m * n * item
+    if max_columns is None:
+        free = _free_device_bytes(L.device)
+        max_columns = int(free * 0.9) // per_column
+        if max_columns < 1:
+            raise ValueError(
+                "The Chebyshev basis of one signal ({0} vectors of {1} x {2} bytes, {3:.2f} GB) "
+                "does not fit in the free device memory ({4:.2f} GB). Lower the order.".format(
+                    m, n, item, per_column / 2 ** 30, free / 2 ** 30))
+    step = max(1, min(int(max_columns), nsig))
+    cd = torch.as_tensor(c, device=L.device)
+    basis = torch.empty((m, n, step), dtype=L.dtype, device=L.device)
+    with torch.cuda.device(L.device):
+        for j0 in range(0, nsig, step):
+            j1 = min(nsig, j0 + step)
+            b = j1 - j0
+            if b == nsig:
+                buf, xc = basis, x
+            else:
+                # the chunk is staged in slot 0 of the basis, where the recurrence reads T_0
+                buf = basis.view(-1)[:m * n * b].view(m, n, b)
+                buf[0].copy_(x[:, j0:j1])
+                xc = buf[0]
+            nat.call("gsp_cheby_op_basis_" + nat.suffix(L.dtype), nat.i64(n), nat.i64(L.nnz),
+                     L.indptr, L.indices, L.data, nat.f64(lmax), cd, nat.i32(nf), nat.i32(m), xc,
+                     nat.i64(b), buf, out[:, :, j0:], nat.i64(nsig), L.tile_plan(b, 0),
+                     nat.stream_ptr(L.device))
+    return out
+
+
+def cheby_synthesis_wide_device(L, lmax, c, sources):
+    """sum_f p_f(L) s_f for any number of source blocks, device to device: (N, nsig).
+
+    ``sources`` is (nsrc, N, nsig), ``c`` (nsrc, M).  One mix pass forms the per-order sources
+    u_k = sum_f c_fk s_f (c_f0 halved) and ONE Clenshaw recurrence runs with the source of order k
+    (csrc/cheby_bank.cu, ``gsp_cheby_synthesis_wide_*``): K SpMMs, where the reference's synthesis
+    runs nsrc forward recurrences (filter.py:313-322).  Same value as
+    :func:`cheby_clenshaw_device`, different rounding.  Work memory: (M + 2) N nsig elements."""
+    torch = nat.require_cuda()
+    c = np.ascontiguousarray(np.atleast_2d(np.asarray(c, dtype=np.float64)))
+    nsrc, m = c.shape
+    if m < 2:
+        raise TypeError("The coefficients have an invalid shape")
+    if sources.dim() == 2:
+        sources = sources[None]
+    if sources.shape[0] != nsrc:
+        raise ValueError("one coefficient row per source block")
+    sources = sources.contiguous()
+    _, n, nsig = sources.shape
+    out = torch.empty((n, nsig), dtype=L.dtype, device=L.device)
+    if n == 0 or nsig == 0:
+        return out
+    work = torch.empty((m + 2, n, nsig), dtype=L.dtype, device=L.device)
+    cd = torch.as_tensor(c, device=L.device)
+    with torch.cuda.device(L.device):
+        nat.call("gsp_cheby_synthesis_wide_" + nat.suffix(L.dtype), nat.i64(n), nat.i64(L.nnz),
+                 L.indptr, L.indices, L.data, nat.f64(lmax), cd, nat.i32(nsrc), nat.i32(m),
+                 sources, nat.i64(nsig), out, work, L.tile_plan(nsig, 1), nat.stream_ptr(L.device))
+    return out
+
+
 def cheby_clenshaw_device(L, lmax, c, sources, out=None, work=None):
     """sum_i p_i(L) s_i by ONE backward (Clenshaw) recurrence, device to device.
 
@@ -204,6 +295,8 @@ def cheby_op(G, c, signal, **kwargs):
         clenshaw = c.shape[0] == 1
     if clenshaw:
         r = cheby_clenshaw_device(L, G.lmax, c[0], x)
+    elif c.shape[0] > WIDE_BANK:
+        r = cheby_bank_device(L, G.lmax, c, x)
     else:
         r = cheby_op_device(L, G.lmax, c, x)
     r = r.reshape(c.shape[0] * G.N, x.shape[1])

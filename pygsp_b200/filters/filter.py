@@ -126,14 +126,19 @@ class Filter:
             x, _, kind = approximations._as_device_block(view, flat)
             if self.clenshaw and c.shape[0] == 1:
                 r = approximations.cheby_clenshaw_device(L, self.G.lmax, c, x)[None]
+            elif c.shape[0] > approximations.WIDE_BANK:
+                r = approximations.cheby_bank_device(L, self.G.lmax, c, x)
             else:
                 r = approximations.cheby_op_device(L, self.G.lmax, c, x)  # (Nf, N, nsig)
             out = r.permute(1, 2, 0)                                      # (N, nsig, Nf)
         else:                                                    # synthesis
             x, _, kind = approximations._as_device_block(view, s.reshape(N, -1))
             x = x.reshape(N, n_signals, n_features_in)
-            if self.fused_synthesis and n_features_in <= 16:
+            if self.fused_synthesis and n_features_in <= approximations.WIDE_BANK:
                 out = approximations.cheby_clenshaw_device(L, self.G.lmax, c, x.permute(2, 0, 1))
+            elif self.fused_synthesis:
+                out = approximations.cheby_synthesis_wide_device(L, self.G.lmax, c,
+                                                                 x.permute(2, 0, 1))
             else:
                 out = torch.zeros((N, n_signals), dtype=L.dtype, device=L.device)
                 for i in range(n_features_in):
@@ -186,8 +191,69 @@ class Filter:
         s = np.identity(self.G.N)
         return self.filter(s, **kwargs).T.reshape(-1, self.G.N)
 
+    def toarray(self):
+        r"""Array representation of the bank: :meth:`compute_frame` (filter.py:105-110)."""
+        return self.compute_frame()
+
     def localize(self, i, **kwargs):
         r"""Kernels localised at vertex ``i``: sqrt(N) g(L) delta_i (filter.py:350-391)."""
         delta = np.zeros(self.G.N)
         delta[i] = 1
         return self.filter(delta, **kwargs) * np.sqrt(self.G.N)
+
+    # ------------------------------------------------------------------------ frames
+    def estimate_frame_bounds(self, x=None):
+        r"""Frame bounds (A, B): the extrema over ``x`` of ``sum_i g_i(x)^2`` (filter.py:393-504).
+
+        ``x`` defaults to 1000 evenly spaced points of [0, lmax]; pass ``G.e`` for the exact
+        bounds on the graph's spectrum.  Host NumPy on the responses.
+        """
+        x = np.linspace(0, self.G.lmax, 1000) if x is None else np.asanyarray(x)
+        energy = np.sum(self.evaluate(x) ** 2, axis=0)
+        return energy.min(), energy.max()
+
+    def complement(self, frame_bound=None):
+        r"""The filter that makes the bank a tight frame: ``sqrt(B - sum_i g_i(x)^2)``
+        (filter.py:602-661).
+
+        ``B`` is ``frame_bound``, or the largest energy among the frequencies the complement is
+        evaluated at when it is None.  A bound below that energy raises ``ValueError`` when the
+        complement is evaluated.
+        """
+        def kernel(x):
+            energy = np.sum(self.evaluate(x) ** 2, axis=0)
+            peak = energy.max()
+            if frame_bound is None:
+                bound = peak
+            elif peak > frame_bound:
+                raise ValueError("The chosen bound is not feasible. "
+                                 "Choose at least {}.".format(peak))
+            else:
+                bound = frame_bound
+            return np.sqrt(bound - energy)
+
+        return Filter(self.G, kernel)
+
+    def inverse(self):
+        r"""The bank whose synthesis inverts this bank's analysis (filter.py:663-759).
+
+        At every frequency the responses h(x) of the inverse are the pseudo-inverse of the column
+        g(x) of this bank's responses: ``h_i(x) = g_i(x) / sum_j g_j(x)^2``, and 0 where every
+        g_j(x) is 0.  A warning is logged when the frame bounds (on [0, lmax]) say the bank is not
+        a frame (A = 0) or is badly conditioned (A / B < 1e-10).
+        """
+        A, B = self.estimate_frame_bounds()
+        if A == 0:
+            _logger.warning("The filter bank is not invertible as it is not "
+                            "a frame (lower frame bound A=0).")
+        elif A / B < 1e-10:
+            _logger.warning("The filter bank is badly conditioned. "
+                            "The inverse will be approximate.")
+
+        def kernel(x, i):
+            g = self.evaluate(x)
+            energy = np.sum(g ** 2, axis=0)
+            safe = np.where(energy > 0, energy, 1.0)
+            return np.where(energy > 0, g[i] / safe, 0.0)
+
+        return Filter(self.G, [lambda x, i=i: kernel(x, i) for i in range(self.n_filters)])
