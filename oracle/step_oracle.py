@@ -7,6 +7,9 @@ TEST INFRASTRUCTURE ONLY: nothing under ``pygsp_b200/`` imports this module.
     x_new = alpha * (L x_cur) + beta * x_cur + gamma * x_old          (first: no gamma term)
     r_k   = r_k + ck[k] * x_new        (first: r_k = c0[k]/2 * x_cur + ck[k] * x_new)
 
+or, in the Clenshaw form (``add_source``), x_new = x_new + sum_i cs[i] * s_i with read-only source
+blocks s_i and no accumulator.
+
 :func:`step_reference` evaluates the same step in a wider type than the engine's (float64 for
 a float32 engine, ``np.longdouble`` for a float64 one) from the engine's own input values and
 from the coefficients rounded to the engine type exactly as the kernels round them
@@ -44,13 +47,19 @@ def _csr_products(L, x, work):
     return S, A
 
 
-def step_reference(L, x_cur, x_old, r, alpha, beta, gamma, ck, c0, first, dtype=np.float32):
+def step_reference(L, x_cur, x_old, r, alpha, beta, gamma, ck, c0, first, dtype=np.float32,
+                   sources=None, cs=None):
     r"""One ``gsp_cheby_step_*`` on all rows of the square CSR ``L`` (values in the engine dtype).
 
     ``x_cur``, ``x_old``: (n, nsig) in the engine dtype (``x_old`` ignored when ``first``); ``r``:
     (nscales, n, nsig) accumulators before the step (ignored when ``first``); ``ck``, ``c0``: the
     float64 coefficients handed to the library.  Returns ``(x_new, r_new, bound_x, bound_r)``,
     references in the wide type and bounds in float64, shapes (n, nsig) and (nscales, n, nsig).
+
+    ``sources`` (nsrc, n, nsig) in the engine dtype and ``cs`` (nsrc float64 coefficients) model
+    the Clenshaw form of the step: after the three operations below, ``x_new = fma(c_i, s_i,
+    x_new)`` for i = 0 .. nsrc-1 in that order, and no accumulator (``r`` must be None; r_new and
+    bound_r have nscales = 0).  Without ``sources`` the results are those of the plain step.
 
     Derivation.  u is the engine's unit roundoff (2^-24 float32, 2^-53 float64) and every
     operation of the kernel obeys fl(z) = z (1 + d), |d| <= u, plus an absolute error <= eta
@@ -83,6 +92,17 @@ def step_reference(L, x_cur, x_old, r, alpha, beta, gamma, ck, c0, first, dtype=
         |r - R| <= (1+u) |c| |x_new - X| + u |c| M + gamma_2 |h x_c|
                 <= gamma_{m'+2} |c| M + gamma_2 |h x_c|.
 
+    Sources (Clenshaw form), c_i = cs[i] rounded to the engine type, Z = sum_i |c_i s_i| and
+    x^(0) the x_new above: x^(i+1) = (x^(i) + c_i s_i)(1 + d_i), exact target E = X + sum_i c_i s_i.
+    Unrolled, x^(nsrc) = x^(0) prod_i (1 + d_i) + sum_i c_i s_i prod_{j>=i} (1 + d_j), so
+
+        |x^(nsrc) - E| <= (1 + gamma_nsrc) |x^(0) - X| + gamma_nsrc (|X| + Z)
+                       <= gamma_{m'+2+nsrc} (M + Z)          (first: gamma_{m'+1+nsrc} (M + Z)),
+
+    using |X| <= M and (1 + gamma_j)(1 + gamma_k) <= 1 + gamma_{j+k}.  Each fma adds at most one
+    eta on underflow (the floor counts 2 eta, one smallest subnormal, per source), and the
+    reference, one more rounded sum per source, lies within gamma^w_{m'+3+nsrc} (M + Z) of E.
+
     (The one-rounding terms gamma_1 |r_old| are written gamma_2, which keeps every bound at least
     twice the rounding of the stored result itself, u |R|: the float32 rounding of the exact value
     then sits at most half-way to the bound.  Only these slacks of one u separate the bound
@@ -107,8 +127,10 @@ def step_reference(L, x_cur, x_old, r, alpha, beta, gamma, ck, c0, first, dtype=
     ck = np.atleast_1d(np.asarray(ck, dtype=np.float64))
     c0 = np.atleast_1d(np.asarray(c0, dtype=np.float64))
     nscales = 0 if r is None else int(np.asarray(r).shape[0])
+    if sources is not None and nscales:
+        raise ValueError("the Clenshaw form reads source blocks and writes no accumulator")
     a, b, g = (work(dtype.type(v)) for v in (alpha, beta, gamma))
-    cs = [work(dtype.type(ck[k])) for k in range(nscales)]
+    cks = [work(dtype.type(ck[k])) for k in range(nscales)]
     hs = [work(dtype.type(0.5 * c0[k])) for k in range(nscales)]
 
     S, A = _csr_products(L, x_cur, work)
@@ -124,14 +146,24 @@ def step_reference(L, x_cur, x_old, r, alpha, beta, gamma, ck, c0, first, dtype=
         x_new = x_new + g * xo
         Mx = Mx + np.abs(g * xo)
         gx = _gamma(mp + 2, u)
+    nsrc = 0
+    if sources is not None:
+        cw = np.atleast_1d(np.asarray(cs, dtype=np.float64)).astype(dtype).astype(work)
+        nsrc = len(cw)
+        src = np.asarray(sources, dtype=dtype).reshape(nsrc, n, nsig)
+        for i in range(nsrc):
+            t = cw[i] * src[i].astype(work)
+            x_new = x_new + t
+            Mx = Mx + np.abs(t)
+        gx = _gamma((mp + 1 if first else mp + 2) + nsrc, u)
     Mx64 = Mx.astype(np.float64)
-    floor_x = tiny * (m * max(abs(float(a)), 1.0) + 3)
-    bound_x = gx * Mx64 + _gamma(mp + 3, uw) * Mx64 + floor_x
+    floor_x = tiny * (m * max(abs(float(a)), 1.0) + 3 + nsrc)
+    bound_x = gx * Mx64 + _gamma(mp + 3 + nsrc, uw) * Mx64 + floor_x
 
     r_new = np.zeros((nscales, n, nsig), dtype=work)
     bound_r = np.zeros((nscales, n, nsig), dtype=np.float64)
     for k in range(nscales):
-        c = cs[k]
+        c = cks[k]
         if first:
             other = hs[k] * xc
             gc = _gamma(mp + 2, u)
@@ -145,6 +177,42 @@ def step_reference(L, x_cur, x_old, r, alpha, beta, gamma, ck, c0, first, dtype=
                       + max(abs(float(c)), 1.0) * floor_x + 2 * tiny)
     scale = 1.0 + 2.0 ** -40
     return x_new, r_new, bound_x * scale, bound_r * scale
+
+
+def mix_reference(sources, c, dtype=np.float32):
+    r"""The per-order sources of the wide synthesis, ``u_k = sum_f c'_fk s_f``, with a bound.
+
+    ``sources``: (nsrc, n, nsig) in the engine dtype; ``c``: (nsrc, m) float64 coefficients, of
+    which the kernel uses c'_fk = T(c_fk) for k > 0 and T(c_f0 / 2) for k = 0.  Returns ``(u,
+    bound)``, shapes (m, n, nsig), the reference in the wide type and the bound in float64.
+
+    Derivation.  The kernel runs ``acc = fma(c'_fk, s_f, acc)`` from acc = 0 in increasing f, so the
+    f-th product passes through nsrc - f roundings and, with Z_k = sum_f |c'_fk s_f|,
+    |u_k - exact| <= gamma_nsrc Z_k, plus eta per fma on underflow (counted as one smallest
+    subnormal per source).  The reference sums the exact products (a product of two engine values
+    is exact in the wide type for float32, and within u_w of it for float64) with one rounding
+    each, within gamma^w_{nsrc+1} Z_k of the exact sum.  Rounded up by 2^-40 like the step's.
+    """
+    dtype = np.dtype(dtype)
+    work = np.float64 if dtype == np.float32 else np.longdouble
+    u = float(np.finfo(dtype).eps) / 2
+    uw = float(np.finfo(work).eps) / 2
+    tiny = float(np.finfo(dtype).smallest_subnormal)
+    c = np.atleast_2d(np.asarray(c, dtype=np.float64)).copy()
+    c[:, 0] *= 0.5
+    cw = c.astype(dtype).astype(work)
+    nsrc, m = c.shape
+    src = np.asarray(sources, dtype=dtype)
+    shape = src.shape[1:]
+    flat = src.reshape(nsrc, -1).astype(work)
+    uk = np.zeros((m, flat.shape[1]), dtype=work)
+    zk = np.zeros((m, flat.shape[1]), dtype=work)
+    for f in range(nsrc):
+        uk += cw[f][:, None] * flat[f][None, :]
+        zk += np.abs(cw[f][:, None] * flat[f][None, :])
+    z = zk.astype(np.float64)
+    bound = (float(_gamma(nsrc, u)) + float(_gamma(nsrc + 1, uw))) * z + tiny * nsrc
+    return uk.reshape((m,) + shape), bound.reshape((m,) + shape) * (1.0 + 2.0 ** -40)
 
 
 def violations(got, ref, bound):

@@ -23,43 +23,51 @@ constexpr int kMixThreads = 256;
 constexpr int kMixFilters = 32;        // coefficient rows staged in shared memory at a time
 
 // r_i = sum_k c_ik T_k x over the elements of a (n, nsig) block, VEC consecutive elements per
-// thread.  The CTA stages the m basis values of its elements in shared memory once (each thread
-// reads back only what it staged, so no barrier is needed) and loops over all nscales filters;
-// the coefficient rows are read from L2 as doubles.  The chain is the fused step's, with the
-// coefficients cast to T as StepCoef casts them:
+// thread, for the orders k0 .. k1 - 1 of one chunk.  The CTA stages the basis values of its
+// elements for these orders in shared memory once (each thread reads back only what it staged, so
+// no barrier is needed) and loops over all nscales filters; the coefficient rows are read from L2
+// as doubles.  The chain is the fused step's, with the coefficients cast to T as StepCoef casts
+// them:
 //   r = fma(c_i1, T_1, T(c_i0 / 2) T_0), then r = fma(c_ik, T_k, r) for k = 2 .. m-1
-// so the result is the bits of gsp_cheby_op_* on the same block.
+// so the result is the bits of gsp_cheby_op_* on the same block.  A chunk past the first
+// (k0 > 0) continues the chain from the r the previous chunk stored: r is a T value, so storing
+// and reloading it changes no bit.
 template <typename T, int VEC>
 __global__ void __launch_bounds__(kCombineThreads)
 cheby_basis_combine(int64_t count, int nsig, const T* __restrict__ t0, const T* __restrict__ basis,
-                    int m, const double* __restrict__ coeffs, int nscales, T* __restrict__ r,
-                    int64_t r_stride, int64_t ldr) {
+                    int m, int k0, int k1, const double* __restrict__ coeffs, int nscales,
+                    T* __restrict__ r, int64_t r_stride, int64_t ldr) {
   extern __shared__ __align__(16) unsigned char combine_smem[];
-  Vec<T, VEC>* tile = reinterpret_cast<Vec<T, VEC>*>(combine_smem);   // (m, blockDim.x)
+  Vec<T, VEC>* tile = reinterpret_cast<Vec<T, VEC>*>(combine_smem);   // (k1 - k0, blockDim.x)
   const int tpb = blockDim.x;
   const int64_t e = (int64_t(blockIdx.x) * tpb + threadIdx.x) * VEC;
   if (e >= count) return;
-  Vec<T, VEC>* mine = tile + threadIdx.x;
-  mine[0] = load_vec_stream<T, VEC>(t0 + e);
-  for (int k = 1; k < m; ++k) mine[k * tpb] = load_vec_stream<T, VEC>(basis + int64_t(k) * count + e);
+  Vec<T, VEC>* mine = tile + threadIdx.x;                  // slot k - k0 holds T_k
+  for (int k = k0; k < k1; ++k)
+    mine[(k - k0) * tpb] = load_vec_stream<T, VEC>(k == 0 ? t0 + e : basis + int64_t(k) * count + e);
   const int64_t row = e / nsig;
   T* out = r + row * ldr + (e - row * nsig);
   for (int i = 0; i < nscales; ++i) {
     const double* ci = coeffs + int64_t(i) * m;
-    const T h0 = T(0.5 * __ldg(ci));
-    const T c1 = T(__ldg(ci + 1));
-    const Vec<T, VEC> x0 = mine[0], x1 = mine[tpb];
+    T* oi = out + int64_t(i) * r_stride;
     Vec<T, VEC> acc;
+    if (k0 == 0) {
+      const T h0 = T(0.5 * __ldg(ci));
+      const T c1 = T(__ldg(ci + 1));
+      const Vec<T, VEC> x0 = mine[0], x1 = mine[tpb];
 #pragma unroll
-    for (int v = 0; v < VEC; ++v) acc.v[v] = fma(c1, x1.v[v], h0 * x0.v[v]);
+      for (int v = 0; v < VEC; ++v) acc.v[v] = fma(c1, x1.v[v], h0 * x0.v[v]);
+    } else {
+      acc = load_vec_stream<T, VEC>(oi);
+    }
 #pragma unroll 4
-    for (int k = 2; k < m; ++k) {
+    for (int k = max(k0, 2); k < k1; ++k) {
       const T ck = T(__ldg(ci + k));
-      const Vec<T, VEC> xk = mine[k * tpb];
+      const Vec<T, VEC> xk = mine[(k - k0) * tpb];
 #pragma unroll
       for (int v = 0; v < VEC; ++v) acc.v[v] = fma(ck, xk.v[v], acc.v[v]);
     }
-    store_vec_stream<T, VEC>(out + int64_t(i) * r_stride, acc);
+    store_vec_stream<T, VEC>(oi, acc);
   }
 }
 
@@ -103,6 +111,10 @@ cheby_mix_orders(int64_t count, const T* __restrict__ src, int nsrc, const doubl
     if (k < kn) __stcs(u + int64_t(k0 + k) * count + e, acc[k]);
 }
 
+// The combine in order chunks.  The thread count halves from 128 to 32 while the m staged values of
+// a thread do not fit in the shared-memory opt-in (m <= 113, 227, 454 at 16 B per value, the
+// vectorised case in both types); past that the orders are split into chunks of as many as fit
+// at 32 threads, each launch continuing the chains of the one before.
 template <typename T, int VEC>
 static int launch_combine(int64_t count, int nsig, const T* t0, const T* basis, int m,
                           const double* coeffs, int nscales, T* r, int64_t r_stride, int64_t ldr,
@@ -110,19 +122,22 @@ static int launch_combine(int64_t count, int nsig, const T* t0, const T* basis, 
   int dev = 0, optin = 0;
   GSP_CUDA(cudaGetDevice(&dev));
   GSP_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-  const int64_t per_thread = int64_t(m) * VEC * sizeof(T);
+  const int64_t per_order = int64_t(VEC) * sizeof(T);      // bytes per thread and order
   int tpb = kCombineThreads;
-  while (tpb > 32 && per_thread * tpb > optin) tpb /= 2;
-  if (per_thread * tpb > optin)
-    return fail(GSP_ERR_UNSUPPORTED, "basis combine: the order is too high for one shared-memory tile");
-  const size_t smem = size_t(per_thread) * tpb;
+  while (tpb > 32 && per_order * m * tpb > optin) tpb /= 2;
+  const int chunk = int(std::min<int64_t>(m, optin / (per_order * tpb)));
+  GSP_REQUIRE(chunk >= 2, "basis combine: no shared memory for two orders");
+  const size_t smem = size_t(per_order) * chunk * tpb;
   GSP_CUDA(cudaFuncSetAttribute(cheby_basis_combine<T, VEC>,
                                 cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int64_t blocks = ceil_div(count, int64_t(tpb) * VEC);
   GSP_REQUIRE(blocks < (int64_t(1) << 31), "block too large for one combine launch");
-  cheby_basis_combine<T, VEC><<<(unsigned)blocks, tpb, smem, st>>>(count, nsig, t0, basis, m, coeffs,
-                                                                  nscales, r, r_stride, ldr);
-  GSP_LAUNCH_CHECK("cheby_basis_combine");
+  for (int k0 = 0; k0 < m; k0 += chunk) {
+    const int k1 = std::min(m, k0 + chunk);
+    cheby_basis_combine<T, VEC><<<(unsigned)blocks, tpb, size_t(per_order) * (k1 - k0) * tpb, st>>>(
+        count, nsig, t0, basis, m, k0, k1, coeffs, nscales, r, r_stride, ldr);
+    GSP_LAUNCH_CHECK("cheby_basis_combine");
+  }
   return GSP_OK;
 }
 

@@ -319,7 +319,9 @@ def test_cheby_op_signal_widths(gsp, sensor5k, nsig):
 
 @pytest.mark.parametrize("nscales,nsig", [(1, 64), (2, 8), (6, 64), (6, 3), (17, 4), (33, 1)])
 def test_cheby_op_filter_banks(gsp, sensor5k, nscales, nsig):
-    """Banks wider than the 16 coefficients a launch carries take the axpy path."""
+    """Banks of 1 to 33 filters through the public cheby_op: up to 16 the fused step, wider
+    banks the stored-basis route (cheby_bank_device).  The fused step's axpy path for more than
+    16 scales (cheby_axpy_scales) is tested directly in test_filter_banks_gpu.py."""
     G, L, _ = sensor5k
     rng = np.random.default_rng(1000 + nscales)
     x = rng.standard_normal((G.N, nsig))
