@@ -11,9 +11,12 @@
  *   - return value 0 = OK, negative = error (-1 bad argument, -2 CUDA error,
  *     -3 unsupported); the message is available from gsp_last_error()
  *     (thread-local).  Nothing throws across the boundary;
- *   - the callee never frees or keeps caller memory.  Outputs whose size is
- *     data dependent come as a *_count / *_fill pair: the count pass writes
- *     the output indptr (whose last element is the nnz to allocate);
+ *   - the callee never frees or keeps caller memory.  A CSR output whose size
+ *     is data dependent comes as a *_count / *_fill pair.  The count writes
+ *     the output indptr and, through its `int64_t* nnz` argument (device, may
+ *     be NULL), the number of entries as an int64; indptr is meaningful only
+ *     when *nnz < 2^31, which the caller checks before it allocates the fill's
+ *     outputs;
  *   - CSR index arrays are int32 (as SciPy's for nnz < 2^31), values are
  *     float (_f32) or double (_f64); the weighted degree `dw` is always double.
  */
@@ -27,7 +30,7 @@
 extern "C" {
 #endif
 
-#define GSPB200_ABI_VERSION 2
+#define GSPB200_ABI_VERSION 3
 
 int gsp_abi_version(void);
 const char* gsp_last_error(void);
@@ -629,7 +632,7 @@ int gsp_cheby_op_dist_phases_f64(const gsp_dist_plan* plan_host, const gsp_tile_
  * gsp_knn_to_csr_*: directed k-NN matrix W[i, nn] = exp(-d^2/sigma) as CSR with sorted
  *     rows (nngraph.py:221-226,289); symmetrise with gsp_csr_transpose / _average.
  */
-int gsp_grid2d_count(int64_t n1, int64_t n2, int32_t* indptr, void* stream);
+int gsp_grid2d_count(int64_t n1, int64_t n2, int32_t* indptr, int64_t* nnz, void* stream);
 int gsp_grid2d_fill_f32(int64_t n1, int64_t n2, const int32_t* indptr, int32_t* indices,
                         float* data, void* stream);
 int gsp_grid2d_fill_f64(int64_t n1, int64_t n2, const int32_t* indptr, int32_t* indices,
@@ -653,10 +656,8 @@ int gsp_knn_to_csr_f64(int64_t n, int k, const int32_t* nn_idx, const double* nn
  *     any d.  1 <= k <= 32, k < n.  Outputs (n, k) like gsp_knn_grid: ascending (distance, id),
  *     independent of the launch configuration.
  * gsp_radius_count / gsp_radius_fill_f64: nngraph.py:228-283, query_ball_point(r = epsilon, p)
- *     and the j != i filter: row i = {j != i : dist(x_i, x_j) <= epsilon}.  count writes indptr
- *     (n + 1) and the number of entries to *nnz (device int64); indptr is meaningful only when
- *     *nnz < 2^31, which the caller checks before allocating.  fill writes the columns (sorted,
- *     bit-identical from run to run) and their distances (double).
+ *     and the j != i filter: row i = {j != i : dist(x_i, x_j) <= epsilon}.  fill writes the
+ *     columns (sorted, bit-identical from run to run) and their distances (double).
  * gsp_csr_symmetrize_count_* / _fill_*: utils.py:244-277 symmetrize(W, method) for mode
  *     0 'maximum' (W - W o [W^T > W] + W^T o [W^T > W]), 1 'fill' (W + ((A + A^T) - A) o W^T,
  *     A = W > 0, then 'average'), 2 'tril' and 3 'triu' (one triangle, then 'maximum').  A is W,
@@ -674,7 +675,8 @@ int gsp_radius_fill_f64(int64_t n, int d, const double* points, double epsilon, 
   int gsp_csr_symmetrize_count_##SUF(int64_t n, int mode, const int32_t* a_indptr,               \
                                      const int32_t* a_indices, const T* a_data,                  \
                                      const int32_t* b_indptr, const int32_t* b_indices,          \
-                                     const T* b_data, int32_t* s_indptr, void* stream);          \
+                                     const T* b_data, int32_t* s_indptr, int64_t* nnz,           \
+                                     void* stream);                                              \
   int gsp_csr_symmetrize_fill_##SUF(int64_t n, int mode, const int32_t* a_indptr,                \
                                     const int32_t* a_indices, const T* a_data,                   \
                                     const int32_t* b_indptr, const int32_t* b_indices,           \
@@ -718,7 +720,7 @@ GSPB200_DECLARE_LAYOUT_API(f64, double)
   int gsp_csr_inspect_##SUF(int64_t n, const int32_t* indptr, const int32_t* indices,            \
                             const T* data, int64_t* stats_dev, void* stream);                    \
   int gsp_csr_compact_count_##SUF(int64_t n, const int32_t* indptr, const T* data,               \
-                                  int32_t* out_indptr, void* stream);                            \
+                                  int32_t* out_indptr, int64_t* nnz, void* stream);              \
   int gsp_csr_compact_fill_##SUF(int64_t n, const int32_t* indptr, const int32_t* indices,       \
                                  const T* data, const int32_t* out_indptr, int32_t* out_indices, \
                                  T* out_data, void* stream);                                     \
@@ -733,7 +735,7 @@ GSPB200_DECLARE_LAYOUT_API(f64, double)
   int gsp_csr_average_count_##SUF(int64_t n, const int32_t* a_indptr, const int32_t* a_indices,  \
                                   const T* a_data, const int32_t* b_indptr,                      \
                                   const int32_t* b_indices, const T* b_data, int32_t* s_indptr,  \
-                                  void* stream);                                                 \
+                                  int64_t* nnz, void* stream);                                   \
   int gsp_csr_average_fill_##SUF(int64_t n, const int32_t* a_indptr, const int32_t* a_indices,   \
                                  const T* a_data, const int32_t* b_indptr,                       \
                                  const int32_t* b_indices, const T* b_data,                      \
@@ -744,7 +746,7 @@ GSPB200_DECLARE_LAYOUT_API(f64, double)
                        void* stream);                                                            \
   int gsp_laplacian_count_##SUF(int64_t n, const int32_t* indptr, const int32_t* indices,        \
                                 const T* data, const double* dw, int lap_type,                   \
-                                int32_t* l_indptr, void* stream);                                \
+                                int32_t* l_indptr, int64_t* nnz, void* stream);                  \
   int gsp_laplacian_fill_##SUF(int64_t n, const int32_t* indptr, const int32_t* indices,         \
                                const T* data, const double* dw, int lap_type,                    \
                                const int32_t* l_indptr, int32_t* l_indices, T* l_data,           \
@@ -786,7 +788,7 @@ int gsp_edge_offsets(int64_t n, const int32_t* indptr, const int32_t* indices, i
                      void* stream);
 int gsp_incidence_count(int64_t n, const int32_t* indptr, const int32_t* indices,
                         const int32_t* t_indptr, const int32_t* t_indices, int32_t* d_indptr,
-                        void* stream);
+                        int64_t* nnz, void* stream);
 
 #define GSPB200_DECLARE_DIFF_API(SUF, T)                                                         \
   int gsp_edge_list_##SUF(int64_t n, int64_t n_edges, const int32_t* indptr,                     \
@@ -825,10 +827,8 @@ GSPB200_DECLARE_DIFF_API(f64, double)
  *     mpos[mptr[u] .. mptr[u + 1]) are the positions p with v[p] == u, increasing; mptr has
  *     n + 1 entries, mpos m.
  * gsp_subgraph_count / gsp_subgraph_fill_*: W[v, :][:, v] (:247) as CSR (m x m).  labels (may be
- *     NULL) keeps an entry (u, c) only when labels[u] == labels[c].  count writes s_indptr
- *     (m + 1) and the number of entries to *nnz (device); s_indptr is meaningful only when
- *     *nnz < 2^31, which the caller checks before allocating.  fill writes the entries, each row
- *     in W's column order mapped through mpos: sorted when v is strictly increasing, and
+ *     NULL) keeps an entry (u, c) only when labels[u] == labels[c].  fill writes the entries,
+ *     each row in W's column order mapped through mpos: sorted when v is strictly increasing, and
  *     block-diagonal sorted when v lists the vertices by (label, id) and labels is given.
  *     Otherwise the caller sorts the rows (s_rows, may be NULL, receives each entry's row for
  *     gsp_coo_to_csr_*); no two entries coincide.
@@ -933,8 +933,7 @@ int gsp_barabasi_albert(int64_t n, int64_t m0, int64_t m, uint64_t key, int32_t*
 
 /* ------------------------------------------------------------- structured graphs ---
  * The closed-form models of pygsp/graphs/{path,comet,star,torus,fullconnected,randomring}.py as
- * canonical CSR: each count writes indptr (n + 1, row sizes then their scan), each fill the
- * rows.  The caller checks that the result holds fewer than 2^31 entries before allocating.
+ * canonical CSR: each count writes indptr (n + 1) and the total, each fill the rows.
  * gsp_comet_*: star 0 - 1..k and tail path k - ... - n-1 (comet.py); k = 0 is the path graph
  *   (path.py), k = n - 1 the star (star.py); directed != 0 (k = 0 only): edges i -> i+1.  Unit
  *   weights.
@@ -942,7 +941,7 @@ int gsp_barabasi_albert(int64_t n, int64_t m0, int64_t m, uint64_t key, int32_t*
  *   i +- 1 (mod mv); coinciding neighbours are one entry whose weight counts them (2 when
  *   nv <= 2 or mv <= 2, self-loops when nv = 1 or mv = 1), as the reference sums its duplicates.
  * gsp_full_connected_indptr / _fill_*: fullconnected.py, every j != i with weight 1;
- *   n (n - 1) < 2^31.
+ *   n (n - 1) < 2^31.  The indptr call is the count; *nnz is n (n - 1).
  * gsp_random_ring_count / _fill_*: randomring.py on sorted angles (n >= 3, double): the edge
  *   i - i+1 and the closing edge 0 - n-1 have weight width / (angle difference), the closing
  *   difference (2 pi + a[0]) - a[n - 1]; double, rounded once.  Zero differences are not stored.
@@ -951,14 +950,15 @@ int gsp_barabasi_albert(int64_t n, int64_t m0, int64_t m, uint64_t key, int32_t*
  * gsp_line_graph_count / _fill_*: linegraph.py, (D != 0)^T (D != 0) - I (n_edges x n_edges) from
  *   the edge list (sources, targets; gsp_edge_list_*) and D's indptr / indices
  *   (gsp_incidence_fill_*).  w_indptr / w_indices is W, searched for the reciprocal edge t -> s
- *   when directed != 0.  count writes lg_indptr and the total to *nnz (device, int64);
- *   lg_indptr is meaningful only when *nnz < 2^31.  fill writes each row sorted: value 1 for
- *   every edge sharing an end with edge k, or the single entry (k, k) = -1 for a self-loop.
+ *   when directed != 0.  fill writes each row sorted: value 1 for every edge sharing an end with
+ *   edge k, or the single entry (k, k) = -1 for a self-loop.
  */
-int gsp_comet_count(int64_t n, int64_t k, int directed, int32_t* indptr, void* stream);
-int gsp_torus_count(int64_t nv, int64_t mv, int32_t* indptr, void* stream);
-int gsp_full_connected_indptr(int64_t n, int32_t* indptr, void* stream);
-int gsp_random_ring_count(int64_t n, const double* angles, int32_t* indptr, void* stream);
+int gsp_comet_count(int64_t n, int64_t k, int directed, int32_t* indptr, int64_t* nnz,
+                    void* stream);
+int gsp_torus_count(int64_t nv, int64_t mv, int32_t* indptr, int64_t* nnz, void* stream);
+int gsp_full_connected_indptr(int64_t n, int32_t* indptr, int64_t* nnz, void* stream);
+int gsp_random_ring_count(int64_t n, const double* angles, int32_t* indptr, int64_t* nnz,
+                          void* stream);
 int gsp_low_stretch_tree_coo(int levels, int32_t* rows, int32_t* cols, void* stream);
 int gsp_line_graph_count(int64_t n_edges, const int32_t* sources, const int32_t* targets,
                          const int32_t* d_indptr, const int32_t* w_indptr,

@@ -98,7 +98,7 @@ def lib():
             raise NativeError("cannot load %s: %s" % (path, exc))
         _lib.gsp_last_error.restype = ctypes.c_char_p
         _lib.gsp_abi_version.restype = ctypes.c_int
-        if _lib.gsp_abi_version() != 2:
+        if _lib.gsp_abi_version() != 3:
             raise NativeError("libgspb200 ABI mismatch")
     return _lib
 

@@ -94,8 +94,10 @@ inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 // number of SMs of the current device (cached per device)
 int sm_count();
 
-// indptr[1..n] (row sizes on entry) := their inclusive scan, indptr[0] = 0 -- csrc/graph.cu
-int scan_rows(int32_t* indptr, int64_t n, cudaStream_t st);
+// indptr[1..n] (row sizes on entry) := their inclusive scan, indptr[0] = 0.  When nnz (device)
+// is not null it first receives the int64 sum of the row sizes, which stays exact where the int32
+// scan wraps -- csrc/graph.cu
+int scan_rows(int32_t* indptr, int64_t n, int64_t* nnz, cudaStream_t st);
 
 // dst[i,:] = src[idx[i],:] (scatter: dst[idx[i],:] = src[i,:]) -- csrc/graph.cu
 template <typename T>

@@ -152,24 +152,20 @@ __global__ void subgraph_count_kernel(int64_t m, const int32_t* __restrict__ ind
                                       const int32_t* __restrict__ indices,
                                       const int32_t* __restrict__ v,
                                       const int32_t* __restrict__ mptr,
-                                      const int32_t* __restrict__ labels, int32_t* s_indptr,
-                                      unsigned long long* nnz) {
+                                      const int32_t* __restrict__ labels, int32_t* s_indptr) {
   const int64_t r = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
   if (r == 0) s_indptr[0] = 0;
-  long long s = 0;
-  if (r < m) {
-    const int u = __ldg(v + r);
-    const int lu = labels ? __ldg(labels + u) : 0;
-    const int end = __ldg(indptr + u + 1);
-    for (int k = __ldg(indptr + u); k < end; ++k) {
-      const int c = __ldg(indices + k);
-      if (labels && __ldg(labels + c) != lu) continue;
-      s += __ldg(mptr + c + 1) - __ldg(mptr + c);
-    }
-    s_indptr[r + 1] = (int32_t)s;          // at most m < 2^31
+  if (r >= m) return;
+  const int u = __ldg(v + r);
+  const int lu = labels ? __ldg(labels + u) : 0;
+  const int end = __ldg(indptr + u + 1);
+  int s = 0;                               // at most m < 2^31: the columns of a row are distinct
+  for (int k = __ldg(indptr + u); k < end; ++k) {
+    const int c = __ldg(indices + k);
+    if (labels && __ldg(labels + c) != lu) continue;
+    s += __ldg(mptr + c + 1) - __ldg(mptr + c);
   }
-  for (int o = 16; o > 0; o >>= 1) s += __shfl_down_sync(0xffffffffu, s, o);
-  if ((threadIdx.x & 31) == 0 && s) atomicAdd(nnz, (unsigned long long)s);
+  s_indptr[r + 1] = s;
 }
 
 template <typename T>
@@ -276,7 +272,7 @@ int vertex_map(int64_t n, int64_t m, const int32_t* v, int32_t* mptr, int32_t* m
   if (m == 0) return GSP_OK;
   vertex_count_kernel<<<conn_blocks(m), kConnThreads, 0, st>>>(m, v, mptr);
   GSP_LAUNCH_CHECK("vertex_count");
-  int rc = scan_rows(mptr, n, st);
+  int rc = scan_rows(mptr, n, nullptr, st);
   if (rc != GSP_OK) return rc;
   // positions sorted by old id; the radix sort is stable, so each old id's positions increase
   Scratch<int32_t> pos(st), keys_out(st);
@@ -293,11 +289,10 @@ int vertex_map(int64_t n, int64_t m, const int32_t* v, int32_t* mptr, int32_t* m
 int subgraph_count(int64_t m, const int32_t* indptr, const int32_t* indices, const int32_t* v,
                    const int32_t* mptr, const int32_t* labels, int32_t* s_indptr, int64_t* nnz,
                    cudaStream_t st) {
-  GSP_CUDA(cudaMemsetAsync(nnz, 0, sizeof(int64_t), st));
-  subgraph_count_kernel<<<conn_blocks(m), kConnThreads, 0, st>>>(
-      m, indptr, indices, v, mptr, labels, s_indptr, reinterpret_cast<unsigned long long*>(nnz));
+  subgraph_count_kernel<<<conn_blocks(m), kConnThreads, 0, st>>>(m, indptr, indices, v, mptr,
+                                                                  labels, s_indptr);
   GSP_LAUNCH_CHECK("subgraph_count");
-  return scan_rows(s_indptr, m, st);
+  return scan_rows(s_indptr, m, nnz, st);
 }
 
 template <typename T>
@@ -333,7 +328,7 @@ int component_order(int64_t n, const int32_t* labels, int32_t* perm, int32_t* co
                                            (int)n, 0, key_bits(n), st);
   });
   if (rc != GSP_OK) return rc;
-  rc = scan_rows(rank.get(), n, st);
+  rc = scan_rows(rank.get(), n, nullptr, st);
   if (rc != GSP_OK) return rc;
   component_starts_kernel<<<conn_blocks(n), kConnThreads, 0, st>>>(n, sorted.get(), rank.get(),
                                                                    comp_ptr, n_components);
@@ -397,7 +392,7 @@ int gsp_vertex_map(int64_t n, int64_t m, const int32_t* v, int32_t* mptr, int32_
 int gsp_subgraph_count(int64_t m, const int32_t* indptr, const int32_t* indices, const int32_t* v,
                        const int32_t* mptr, const int32_t* labels, int32_t* s_indptr,
                        int64_t* nnz, void* stream) {
-  GSP_REQUIRE(m >= 0 && m < (int64_t(1) << 31) && nnz, "bad arguments");
+  GSP_REQUIRE(m >= 0 && m < (int64_t(1) << 31), "m out of range");
   return gsp::subgraph_count(m, indptr, indices, v, mptr, labels, s_indptr, nnz,
                              gsp::as_stream(stream));
 }

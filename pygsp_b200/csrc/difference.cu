@@ -182,7 +182,7 @@ int edge_offsets(int64_t n, const int32_t* indptr, const int32_t* indices, int32
                  cudaStream_t st) {
   edge_offsets_kernel<<<diff_blocks(n), kDiffThreads, 0, st>>>(n, indptr, indices, eptr);
   GSP_LAUNCH_CHECK("edge_offsets");
-  return scan_rows(eptr, n, st);
+  return scan_rows(eptr, n, nullptr, st);
 }
 
 template <typename T>
@@ -193,7 +193,7 @@ int edge_list(int64_t n, int64_t ne, const int32_t* indptr, const int32_t* indic
                                                                sources, targets, weights,
                                                                dt_indptr);
   GSP_LAUNCH_CHECK("edge_list");
-  return scan_rows(dt_indptr, ne, st);
+  return scan_rows(dt_indptr, ne, nullptr, st);
 }
 
 template <typename T>
@@ -210,11 +210,11 @@ int incidence_t_fill(int64_t ne, const int32_t* sources, const int32_t* targets,
 
 int incidence_count(int64_t n, const int32_t* indptr, const int32_t* indices,
                     const int32_t* t_indptr, const int32_t* t_indices, int32_t* d_indptr,
-                    cudaStream_t st) {
+                    int64_t* nnz, cudaStream_t st) {
   incidence_count_kernel<<<diff_blocks(n), kDiffThreads, 0, st>>>(n, indptr, indices, t_indptr,
                                                                   t_indices, d_indptr);
   GSP_LAUNCH_CHECK("incidence_count");
-  return scan_rows(d_indptr, n, st);
+  return scan_rows(d_indptr, n, nnz, st);
 }
 
 template <typename T>
@@ -268,9 +268,9 @@ int gsp_edge_offsets(int64_t n, const int32_t* indptr, const int32_t* indices, i
 }
 int gsp_incidence_count(int64_t n, const int32_t* indptr, const int32_t* indices,
                         const int32_t* t_indptr, const int32_t* t_indices, int32_t* d_indptr,
-                        void* stream) {
+                        int64_t* nnz, void* stream) {
   GSP_REQUIRE(n >= 0 && (t_indptr == nullptr) == (t_indices == nullptr), "bad arguments");
-  return gsp::incidence_count(n, indptr, indices, t_indptr, t_indices, d_indptr,
+  return gsp::incidence_count(n, indptr, indices, t_indptr, t_indices, d_indptr, nnz,
                               gsp::as_stream(stream));
 }
 GSP_DIFF_API(f32, float)

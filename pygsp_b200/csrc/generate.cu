@@ -213,12 +213,12 @@ static inline int blocks_for(int64_t n) { return (int)ceil_div(n > 0 ? n : 1, kG
 
 extern "C" {
 
-int gsp_grid2d_count(int64_t n1, int64_t n2, int32_t* indptr, void* stream) {
+int gsp_grid2d_count(int64_t n1, int64_t n2, int32_t* indptr, int64_t* nnz, void* stream) {
   GSP_REQUIRE(n1 >= 1 && n2 >= 1 && n1 * n2 < (int64_t(1) << 31), "grid too large");
   cudaStream_t st = gsp::as_stream(stream);
   gsp::grid2d_count_kernel<<<gsp::blocks_for(n1 * n2), gsp::kGenThreads, 0, st>>>(n1, n2, indptr);
   GSP_LAUNCH_CHECK("grid2d_count");
-  return gsp::scan_rows(indptr, n1 * n2, st);
+  return gsp::scan_rows(indptr, n1 * n2, nnz, st);
 }
 
 int gsp_grid2d_fill_f32(int64_t n1, int64_t n2, const int32_t* indptr, int32_t* indices,

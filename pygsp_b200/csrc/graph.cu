@@ -12,6 +12,7 @@
 // outputs whose size is data dependent use a count pass (row sizes -> scan ->
 // indptr) and a fill pass so that the caller allocates the exact nnz.
 #include <cub/cub.cuh>
+#include <thrust/iterator/transform_iterator.h>
 
 #include "common.cuh"
 #include "gspb200.h"
@@ -43,9 +44,24 @@ __device__ __forceinline__ double warp_max(double v) {
 }
 
 // ---- inclusive scan of row sizes into indptr[1..n] -------------------------
-int scan_rows(int32_t* indptr, int64_t n, cudaStream_t st) {
+struct Widen64 {
+  __host__ __device__ int64_t operator()(int32_t v) const { return v; }
+};
+
+int scan_rows(int32_t* indptr, int64_t n, int64_t* nnz, cudaStream_t st) {
   // indptr[0] = 0 and indptr[1..n] hold row sizes on entry
-  if (n == 0) return GSP_OK;
+  if (n == 0) {
+    if (nnz) GSP_CUDA(cudaMemsetAsync(nnz, 0, sizeof(int64_t), st));
+    return GSP_OK;
+  }
+  if (nnz) {
+    // summed in int64 explicitly, not in whatever accumulator CUB deduces from int32 input
+    const thrust::transform_iterator<Widen64, const int32_t*> sizes(indptr + 1, Widen64());
+    const int rc = cub_temp("cub::DeviceReduce::Sum", st, [&](void* tmp, size_t& bytes) {
+      return cub::DeviceReduce::Sum(tmp, bytes, sizes, nnz, (int)n, st);
+    });
+    if (rc != GSP_OK) return rc;
+  }
   return cub_temp("cub::DeviceScan::InclusiveSum", st, [&](void* tmp, size_t& bytes) {
     return cub::DeviceScan::InclusiveSum(tmp, bytes, indptr + 1, indptr + 1, (int)n, st);
   });
@@ -167,7 +183,7 @@ static int csr_transpose(int64_t n, int64_t nnz, const int32_t* indptr, const in
   if (rc != GSP_OK) return rc;
   transpose_unpack_kernel<<<(int)ceil_div(nnz, 256), 256, 0, st>>>(nnz, keys_out.get(), t_indices);
   GSP_LAUNCH_CHECK("transpose_unpack");
-  return scan_rows(t_indptr, n, st);
+  return scan_rows(t_indptr, n, nullptr, st);
 }
 
 // ---- COO -> canonical CSR (sparse.csr_matrix(coo): duplicates summed, rows sorted) ----
@@ -263,7 +279,7 @@ static int coo_to_csr(int64_t n, int64_t nnz, const int32_t* rows, const int32_t
       host[1], ku.get(), indices, indptr);
   GSP_LAUNCH_CHECK("coo_unpack");
   *n_unique_out = host[1];
-  return scan_rows(indptr, n, st);
+  return scan_rows(indptr, n, nullptr, st);
 }
 
 // ---- S = (A + B)/2 with exact-zero results dropped (utils.py:247-248) ----------
@@ -435,10 +451,11 @@ int csr_inspect(int64_t n, const int32_t* p, const int32_t* i, const T* d, int64
 }
 
 template <typename T>
-int csr_compact_count(int64_t n, const int32_t* p, const T* d, int32_t* out_p, cudaStream_t st) {
+int csr_compact_count(int64_t n, const int32_t* p, const T* d, int32_t* out_p, int64_t* nnz,
+                      cudaStream_t st) {
   csr_nonzero_count_kernel<T><<<row_blocks(n), kRowThreads, 0, st>>>(n, p, d, out_p);
   GSP_LAUNCH_CHECK("csr_compact_count");
-  return scan_rows(out_p, n, st);
+  return scan_rows(out_p, n, nnz, st);
 }
 
 template <typename T>
@@ -464,7 +481,7 @@ int csr_asymmetry(int64_t n, const int32_t* p, const int32_t* i, const T* d, int
 template <typename T>
 int csr_average(bool fill, int64_t n, const int32_t* ap, const int32_t* ai, const T* ad,
                 const int32_t* bp, const int32_t* bi, const T* bd, int32_t* sp, int32_t* si,
-                T* sd, cudaStream_t st) {
+                T* sd, int64_t* nnz, cudaStream_t st) {
   if (fill) {
     if (n == 0) return GSP_OK;
     csr_average_kernel<T, true><<<row_blocks(n), kRowThreads, 0, st>>>(n, ap, ai, ad, bp, bi, bd,
@@ -475,7 +492,7 @@ int csr_average(bool fill, int64_t n, const int32_t* ap, const int32_t* ai, cons
   csr_average_kernel<T, false><<<row_blocks(n), kRowThreads, 0, st>>>(n, ap, ai, ad, bp, bi, bd,
                                                                       sp, nullptr, nullptr);
   GSP_LAUNCH_CHECK("csr_average_count");
-  return scan_rows(sp, n, st);
+  return scan_rows(sp, n, nnz, st);
 }
 
 template <typename T>
@@ -489,7 +506,8 @@ int degree(int64_t n, const int32_t* p, const T* d, const int32_t* tp, const T* 
 
 template <typename T>
 int laplacian(bool fill, int64_t n, const int32_t* p, const int32_t* i, const T* d,
-              const double* dw, int lap_type, int32_t* lp, int32_t* li, T* ld, cudaStream_t st) {
+              const double* dw, int lap_type, int32_t* lp, int32_t* li, T* ld, int64_t* nnz,
+              cudaStream_t st) {
   GSP_REQUIRE(lap_type == 0 || lap_type == 1, "Unknown Laplacian type");
   if (fill) {
     if (n == 0) return GSP_OK;
@@ -501,7 +519,7 @@ int laplacian(bool fill, int64_t n, const int32_t* p, const int32_t* i, const T*
   laplacian_kernel<T, false><<<row_blocks(n), kRowThreads, 0, st>>>(n, p, i, d, dw, lap_type, lp,
                                                                     nullptr, nullptr);
   GSP_LAUNCH_CHECK("laplacian_count");
-  return scan_rows(lp, n, st);
+  return scan_rows(lp, n, nnz, st);
 }
 
 template <typename T>
@@ -546,8 +564,8 @@ template int move_rows<double>(bool, int64_t, const int64_t*, const double*, int
     return gsp::csr_inspect<T>(n, indptr, indices, data, stats_dev, gsp::as_stream(stream));    \
   }                                                                                             \
   int gsp_csr_compact_count_##SUF(int64_t n, const int32_t* indptr, const T* data,              \
-                                  int32_t* out_indptr, void* stream) {                          \
-    return gsp::csr_compact_count<T>(n, indptr, data, out_indptr, gsp::as_stream(stream));      \
+                                  int32_t* out_indptr, int64_t* nnz, void* stream) {            \
+    return gsp::csr_compact_count<T>(n, indptr, data, out_indptr, nnz, gsp::as_stream(stream)); \
   }                                                                                             \
   int gsp_csr_compact_fill_##SUF(int64_t n, const int32_t* indptr, const int32_t* indices,      \
                                  const T* data, const int32_t* out_indptr, int32_t* out_indices, \
@@ -576,9 +594,10 @@ template int move_rows<double>(bool, int64_t, const int64_t*, const double*, int
   int gsp_csr_average_count_##SUF(int64_t n, const int32_t* a_indptr, const int32_t* a_indices, \
                                   const T* a_data, const int32_t* b_indptr,                     \
                                   const int32_t* b_indices, const T* b_data, int32_t* s_indptr, \
-                                  void* stream) {                                               \
+                                  int64_t* nnz, void* stream) {                                 \
     return gsp::csr_average<T>(false, n, a_indptr, a_indices, a_data, b_indptr, b_indices,      \
-                               b_data, s_indptr, nullptr, nullptr, gsp::as_stream(stream));     \
+                               b_data, s_indptr, nullptr, nullptr, nnz,                         \
+                               gsp::as_stream(stream));                                         \
   }                                                                                             \
   int gsp_csr_average_fill_##SUF(int64_t n, const int32_t* a_indptr, const int32_t* a_indices,  \
                                  const T* a_data, const int32_t* b_indptr,                      \
@@ -587,7 +606,7 @@ template int move_rows<double>(bool, int64_t, const int64_t*, const double*, int
                                  void* stream) {                                                \
     return gsp::csr_average<T>(true, n, a_indptr, a_indices, a_data, b_indptr, b_indices,       \
                                b_data, const_cast<int32_t*>(s_indptr), s_indices, s_data,       \
-                               gsp::as_stream(stream));                                         \
+                               nullptr, gsp::as_stream(stream));                                \
   }                                                                                             \
   int gsp_degree_##SUF(int64_t n, const int32_t* indptr, const T* data,                         \
                        const int32_t* t_indptr, const T* t_data, double* dw, double* d,         \
@@ -596,16 +615,16 @@ template int move_rows<double>(bool, int64_t, const int64_t*, const double*, int
   }                                                                                             \
   int gsp_laplacian_count_##SUF(int64_t n, const int32_t* indptr, const int32_t* indices,       \
                                 const T* data, const double* dw, int lap_type,                  \
-                                int32_t* l_indptr, void* stream) {                              \
+                                int32_t* l_indptr, int64_t* nnz, void* stream) {                \
     return gsp::laplacian<T>(false, n, indptr, indices, data, dw, lap_type, l_indptr, nullptr,  \
-                             nullptr, gsp::as_stream(stream));                                  \
+                             nullptr, nnz, gsp::as_stream(stream));                             \
   }                                                                                             \
   int gsp_laplacian_fill_##SUF(int64_t n, const int32_t* indptr, const int32_t* indices,        \
                                const T* data, const double* dw, int lap_type,                   \
                                const int32_t* l_indptr, int32_t* l_indices, T* l_data,          \
                                void* stream) {                                                  \
     return gsp::laplacian<T>(true, n, indptr, indices, data, dw, lap_type,                      \
-                             const_cast<int32_t*>(l_indptr), l_indices, l_data,                 \
+                             const_cast<int32_t*>(l_indptr), l_indices, l_data, nullptr,        \
                              gsp::as_stream(stream));                                           \
   }                                                                                             \
   int gsp_spectral_bounds_##SUF(int64_t n, const int32_t* w_indptr, const int32_t* w_indices,   \

@@ -70,13 +70,12 @@ template <int N>
 __device__ __forceinline__ void cp_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N)); }
 
 // MODE kKnn:   out_idx / out_dist are the (n, k) lists.
-// MODE kCount: indptr[i + 1] = row size, *total += row sizes (int64).
+// MODE kCount: indptr[i + 1] = row size.
 // MODE kFill:  row i is written at indptr[i] into out_idx / out_dist, in column order.
 template <int M, int MODE>
 __global__ void __launch_bounds__(kNbThreads, 2)
     neighbors_kernel(int64_t n, int d, const double* __restrict__ pts, int k, double p,
-                     double eps_acc, int32_t* indptr, int32_t* out_idx, double* out_dist,
-                     unsigned long long* total) {
+                     double eps_acc, int32_t* indptr, int32_t* out_idx, double* out_dist) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   double* sq = reinterpret_cast<double*>(smem_raw);   // [2][kQ][kLd]
   double* sc = sq + 2 * kQ * kLd;                     // [2][kC][kLd]
@@ -200,14 +199,12 @@ __global__ void __launch_bounds__(kNbThreads, 2)
   } else if (MODE == kCount) {
     if (my_q == 0) indptr[0] = 0;
     indptr[my_q + 1] = int32_t(cnt);
-    atomicAdd(total, (unsigned long long)cnt);
   }
 }
 
 template <int MODE>
 int launch_neighbors(int64_t n, int d, const double* pts, int k, double p, double eps_acc,
-                     int32_t* indptr, int32_t* out_idx, double* out_dist,
-                     unsigned long long* total, cudaStream_t st) {
+                     int32_t* indptr, int32_t* out_idx, double* out_dist, cudaStream_t st) {
   const int blocks = (int)ceil_div(n, kQ);
 #define GSP_NB_LAUNCH(M)                                                                        \
   do {                                                                                          \
@@ -215,7 +212,7 @@ int launch_neighbors(int64_t n, int d, const double* pts, int k, double p, doubl
     GSP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,            \
                                   (int)kSmemBytes));                                            \
     kern<<<blocks, kNbThreads, kSmemBytes, st>>>(n, d, pts, k, p, eps_acc, indptr, out_idx,     \
-                                                 out_dist, total);                              \
+                                                 out_dist);                                     \
   } while (0)
   if (p == 1.0) GSP_NB_LAUNCH(kL1);
   else if (p == 2.0) GSP_NB_LAUNCH(kL2);
@@ -286,7 +283,7 @@ __global__ void csr_symmetrize_kernel(int64_t n, int mode, const int32_t* __rest
 template <typename T>
 int csr_symmetrize(bool fill, int64_t n, int mode, const int32_t* ap, const int32_t* ai,
                    const T* ad, const int32_t* bp, const int32_t* bi, const T* bd, int32_t* sp,
-                   int32_t* si, T* sd, cudaStream_t st) {
+                   int32_t* si, T* sd, int64_t* nnz, cudaStream_t st) {
   GSP_REQUIRE(mode >= kSymMaximum && mode <= kSymTriu, "unknown symmetrisation mode");
   const int blocks = (int)ceil_div(n > 0 ? n : 1, 256);
   if (fill) {
@@ -299,7 +296,7 @@ int csr_symmetrize(bool fill, int64_t n, int mode, const int32_t* ap, const int3
   csr_symmetrize_kernel<T, false><<<blocks, 256, 0, st>>>(n, mode, ap, ai, ad, bp, bi, bd, sp,
                                                           nullptr, nullptr);
   GSP_LAUNCH_CHECK("csr_symmetrize_count");
-  return scan_rows(sp, n, st);
+  return scan_rows(sp, n, nnz, st);
 }
 
 // w = exp(-d^2 / sigma), the weights of nngraph.py:221-226, 276-281
@@ -334,7 +331,7 @@ int gsp_knn_brute(int64_t n, int d, const double* points, int k, double p, int32
   GSP_REQUIRE_CLOUD(n, d, p);
   GSP_REQUIRE(k >= 1 && k <= gsp::kMaxNbK && k < n, "k must be in [1, 32] and < n");
   return gsp::launch_neighbors<gsp::kKnn>(n, d, points, k, p, 0.0, nullptr, nn_idx, nn_dist,
-                                          nullptr, gsp::as_stream(stream));
+                                          gsp::as_stream(stream));
 }
 
 int gsp_radius_count(int64_t n, int d, const double* points, double epsilon, double p,
@@ -342,12 +339,10 @@ int gsp_radius_count(int64_t n, int d, const double* points, double epsilon, dou
   GSP_REQUIRE_CLOUD(n, d, p);
   GSP_REQUIRE(epsilon >= 0, "epsilon must be >= 0");
   cudaStream_t st = gsp::as_stream(stream);
-  GSP_CUDA(cudaMemsetAsync(nnz, 0, sizeof(int64_t), st));
   const int rc = gsp::launch_neighbors<gsp::kCount>(
-      n, d, points, 1, p, gsp::radius_key(epsilon, p), indptr, nullptr, nullptr,
-      reinterpret_cast<unsigned long long*>(nnz), st);
+      n, d, points, 1, p, gsp::radius_key(epsilon, p), indptr, nullptr, nullptr, st);
   if (rc != GSP_OK) return rc;
-  return gsp::scan_rows(indptr, n, st);
+  return gsp::scan_rows(indptr, n, nnz, st);
 }
 
 int gsp_radius_fill_f64(int64_t n, int d, const double* points, double epsilon, double p,
@@ -355,7 +350,7 @@ int gsp_radius_fill_f64(int64_t n, int d, const double* points, double epsilon, 
   GSP_REQUIRE_CLOUD(n, d, p);
   GSP_REQUIRE(epsilon >= 0, "epsilon must be >= 0");
   return gsp::launch_neighbors<gsp::kFill>(n, d, points, 1, p, gsp::radius_key(epsilon, p),
-                                           const_cast<int32_t*>(indptr), indices, dist, nullptr,
+                                           const_cast<int32_t*>(indptr), indices, dist,
                                            gsp::as_stream(stream));
 }
 
@@ -363,9 +358,10 @@ int gsp_radius_fill_f64(int64_t n, int d, const double* points, double epsilon, 
   int gsp_csr_symmetrize_count_##SUF(int64_t n, int mode, const int32_t* a_indptr,              \
                                      const int32_t* a_indices, const T* a_data,                 \
                                      const int32_t* b_indptr, const int32_t* b_indices,         \
-                                     const T* b_data, int32_t* s_indptr, void* stream) {        \
+                                     const T* b_data, int32_t* s_indptr, int64_t* nnz,          \
+                                     void* stream) {                                            \
     return gsp::csr_symmetrize<T>(false, n, mode, a_indptr, a_indices, a_data, b_indptr,        \
-                                  b_indices, b_data, s_indptr, nullptr, nullptr,                \
+                                  b_indices, b_data, s_indptr, nullptr, nullptr, nnz,           \
                                   gsp::as_stream(stream));                                      \
   }                                                                                             \
   int gsp_csr_symmetrize_fill_##SUF(int64_t n, int mode, const int32_t* a_indptr,               \
@@ -375,7 +371,7 @@ int gsp_radius_fill_f64(int64_t n, int d, const double* points, double epsilon, 
                                     int32_t* s_indices, T* s_data, void* stream) {              \
     return gsp::csr_symmetrize<T>(true, n, mode, a_indptr, a_indices, a_data, b_indptr,         \
                                   b_indices, b_data, const_cast<int32_t*>(s_indptr),            \
-                                  s_indices, s_data, gsp::as_stream(stream));                   \
+                                  s_indices, s_data, nullptr, gsp::as_stream(stream));          \
   }                                                                                             \
   int gsp_gauss_weights_##SUF(int64_t nnz, const double* dist, double sigma, T* w,              \
                               void* stream) {                                                   \

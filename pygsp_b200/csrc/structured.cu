@@ -122,8 +122,9 @@ __global__ void torus_fill_kernel(int64_t nv, int64_t mv, const int32_t* __restr
 // ----------------------------------------------------------------- FullConnected ---
 // Row i holds every j != i: entry e = i (n - 1) + r has column r + (r >= i).  The caller
 // guarantees n (n - 1) < 2^31.
-__global__ void full_connected_indptr_kernel(int64_t n, int32_t* indptr) {
+__global__ void full_connected_indptr_kernel(int64_t n, int32_t* indptr, int64_t* nnz) {
   const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i == 0 && nnz) *nnz = n * (n - 1);
   if (i <= n) indptr[i] = (int32_t)(i * (n - 1));
 }
 
@@ -252,23 +253,18 @@ __global__ void line_graph_count_kernel(int64_t ne, const int32_t* __restrict__ 
                                         const int32_t* __restrict__ d_indptr,
                                         const int32_t* __restrict__ w_indptr,
                                         const int32_t* __restrict__ w_indices, int directed,
-                                        int32_t* lg_indptr, unsigned long long* nnz) {
+                                        int32_t* lg_indptr) {
   const int64_t k = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
   if (k == 0) lg_indptr[0] = 0;
-  long long c = 0;
-  if (k < ne) {
-    const int s = __ldg(sources + k), t = __ldg(targets + k);
-    if (s == t) {
-      c = 1;
-    } else {
-      c = (long long)(__ldg(d_indptr + s + 1) - __ldg(d_indptr + s)) +
-          (__ldg(d_indptr + t + 1) - __ldg(d_indptr + t)) - 2;
-      if (directed && reciprocal_edge(w_indptr, w_indices, s, t) >= 0) --c;
-    }
-    lg_indptr[k + 1] = (int32_t)c;      // meaningful when the total is < 2^31
+  if (k >= ne) return;
+  const int s = __ldg(sources + k), t = __ldg(targets + k);
+  int c = 1;
+  if (s != t) {                 // |D_s| + |D_t| <= nnz(D) < 2^31
+    c = (__ldg(d_indptr + s + 1) - __ldg(d_indptr + s)) +
+        (__ldg(d_indptr + t + 1) - __ldg(d_indptr + t)) - 2;
+    if (directed && reciprocal_edge(w_indptr, w_indices, s, t) >= 0) --c;
   }
-  for (int o = 16; o > 0; o >>= 1) c += __shfl_down_sync(0xffffffffu, c, o);
-  if ((threadIdx.x & 31) == 0 && c) atomicAdd(nnz, (unsigned long long)c);
+  lg_indptr[k + 1] = c;
 }
 
 // One warp per row.  The merge of A = D_s and B = D_t (A first on ties) is cut into windows of
@@ -326,10 +322,11 @@ line_graph_fill_kernel(int64_t ne, const int32_t* __restrict__ sources,
 }
 
 // ------------------------------------------------------------------ drivers ------
-int comet_count(int64_t n, int64_t k, int directed, int32_t* indptr, cudaStream_t st) {
+int comet_count(int64_t n, int64_t k, int directed, int32_t* indptr, int64_t* nnz,
+                cudaStream_t st) {
   comet_count_kernel<<<struct_blocks(n), kStructThreads, 0, st>>>(n, k, directed, indptr);
   GSP_LAUNCH_CHECK("comet_count");
-  return scan_rows(indptr, n, st);
+  return scan_rows(indptr, n, nnz, st);
 }
 
 template <typename T>
@@ -342,10 +339,10 @@ int comet_fill(int64_t n, int64_t k, int directed, const int32_t* indptr, int32_
   return GSP_OK;
 }
 
-int torus_count(int64_t nv, int64_t mv, int32_t* indptr, cudaStream_t st) {
+int torus_count(int64_t nv, int64_t mv, int32_t* indptr, int64_t* nnz, cudaStream_t st) {
   torus_count_kernel<<<struct_blocks(nv * mv), kStructThreads, 0, st>>>(nv, mv, indptr);
   GSP_LAUNCH_CHECK("torus_count");
-  return scan_rows(indptr, nv * mv, st);
+  return scan_rows(indptr, nv * mv, nnz, st);
 }
 
 template <typename T>
@@ -358,8 +355,8 @@ int torus_fill(int64_t nv, int64_t mv, const int32_t* indptr, int32_t* indices, 
   return GSP_OK;
 }
 
-int full_connected_indptr(int64_t n, int32_t* indptr, cudaStream_t st) {
-  full_connected_indptr_kernel<<<struct_blocks(n + 1), kStructThreads, 0, st>>>(n, indptr);
+int full_connected_indptr(int64_t n, int32_t* indptr, int64_t* nnz, cudaStream_t st) {
+  full_connected_indptr_kernel<<<struct_blocks(n + 1), kStructThreads, 0, st>>>(n, indptr, nnz);
   GSP_LAUNCH_CHECK("full_connected_indptr");
   return GSP_OK;
 }
@@ -374,10 +371,11 @@ int full_connected_fill(int64_t n, int32_t* indices, T* data, cudaStream_t st) {
   return GSP_OK;
 }
 
-int random_ring_count(int64_t n, const double* angles, int32_t* indptr, cudaStream_t st) {
+int random_ring_count(int64_t n, const double* angles, int32_t* indptr, int64_t* nnz,
+                      cudaStream_t st) {
   random_ring_count_kernel<<<struct_blocks(n), kStructThreads, 0, st>>>(n, angles, indptr);
   GSP_LAUNCH_CHECK("random_ring_count");
-  return scan_rows(indptr, n, st);
+  return scan_rows(indptr, n, nnz, st);
 }
 
 template <typename T>
@@ -399,12 +397,10 @@ int low_stretch_tree_coo(int levels, int32_t* rows, int32_t* cols, cudaStream_t 
 int line_graph_count(int64_t ne, const int32_t* sources, const int32_t* targets,
                      const int32_t* d_indptr, const int32_t* w_indptr, const int32_t* w_indices,
                      int directed, int32_t* lg_indptr, int64_t* nnz, cudaStream_t st) {
-  GSP_CUDA(cudaMemsetAsync(nnz, 0, sizeof(int64_t), st));
   line_graph_count_kernel<<<struct_blocks(ne), kStructThreads, 0, st>>>(
-      ne, sources, targets, d_indptr, w_indptr, w_indices, directed, lg_indptr,
-      reinterpret_cast<unsigned long long*>(nnz));
+      ne, sources, targets, d_indptr, w_indptr, w_indices, directed, lg_indptr);
   GSP_LAUNCH_CHECK("line_graph_count");
-  return scan_rows(lg_indptr, ne, st);
+  return scan_rows(lg_indptr, ne, nnz, st);
 }
 
 template <typename T>
@@ -461,22 +457,24 @@ int line_graph_fill(int64_t ne, const int32_t* sources, const int32_t* targets,
   }
 
 extern "C" {
-int gsp_comet_count(int64_t n, int64_t k, int directed, int32_t* indptr, void* stream) {
+int gsp_comet_count(int64_t n, int64_t k, int directed, int32_t* indptr, int64_t* nnz,
+                    void* stream) {
   GSP_REQUIRE(n >= 0 && n < (int64_t(1) << 31) && k >= 0 && (k == 0 || (k < n && !directed)),
               "bad comet shape");
-  return gsp::comet_count(n, k, directed, indptr, gsp::as_stream(stream));
+  return gsp::comet_count(n, k, directed, indptr, nnz, gsp::as_stream(stream));
 }
-int gsp_torus_count(int64_t nv, int64_t mv, int32_t* indptr, void* stream) {
+int gsp_torus_count(int64_t nv, int64_t mv, int32_t* indptr, int64_t* nnz, void* stream) {
   GSP_REQUIRE(nv >= 1 && mv >= 1 && nv * mv < (int64_t(1) << 31), "bad torus shape");
-  return gsp::torus_count(nv, mv, indptr, gsp::as_stream(stream));
+  return gsp::torus_count(nv, mv, indptr, nnz, gsp::as_stream(stream));
 }
-int gsp_full_connected_indptr(int64_t n, int32_t* indptr, void* stream) {
+int gsp_full_connected_indptr(int64_t n, int32_t* indptr, int64_t* nnz, void* stream) {
   GSP_REQUIRE(n >= 0 && n * (n - 1) < (int64_t(1) << 31), "n (n - 1) must be < 2^31");
-  return gsp::full_connected_indptr(n, indptr, gsp::as_stream(stream));
+  return gsp::full_connected_indptr(n, indptr, nnz, gsp::as_stream(stream));
 }
-int gsp_random_ring_count(int64_t n, const double* angles, int32_t* indptr, void* stream) {
+int gsp_random_ring_count(int64_t n, const double* angles, int32_t* indptr, int64_t* nnz,
+                          void* stream) {
   GSP_REQUIRE(n >= 3 && n < (int64_t(1) << 30), "bad ring size");
-  return gsp::random_ring_count(n, angles, indptr, gsp::as_stream(stream));
+  return gsp::random_ring_count(n, angles, indptr, nnz, gsp::as_stream(stream));
 }
 int gsp_low_stretch_tree_coo(int levels, int32_t* rows, int32_t* cols, void* stream) {
   GSP_REQUIRE(levels >= 1 && levels <= 15, "levels must be in 1..15");

@@ -5,9 +5,11 @@ holds ``scipy.sparse.csr_matrix`` objects, graph.py:109,620).  Besides the
 read-only surface of the filtering path (``shape``, ``nnz``, ``dot``,
 ``toarray``, ``diagonal``, ``to_scipy``), this module owns every device
 operation that builds or reshapes CSR structure: assembly from COO triplets
-(``from_coo``), ``transpose``, ``symmetrize``, ``eliminate_zeros``, induced
-submatrices (``induced``), the row id of every entry (:func:`row_ids`) and
-the dense float64 copy (``to_dense``).  The differential operator ``G.D`` is
+(``from_coo``) and from a count / fill pair of entry points (``from_counts``,
+which every matrix of data-dependent size goes through), ``transpose``,
+``symmetrize``, ``eliminate_zeros``, induced submatrices (``induced``), the
+row id of every entry (:func:`row_ids`) and the dense float64 copy
+(``to_dense``).  The differential operator ``G.D`` is
 one too, (N, Ne), with its transpose attached as ``.T`` by the builder
 (graphs/difference.py).
 """
@@ -163,6 +165,35 @@ class DeviceCSR:
         m = int(uniq.value)
         return cls(indptr, indices[:m].contiguous(), data[:m].contiguous(), shape)
 
+    @classmethod
+    def from_counts(cls, shape, dtype, device, count, fill, what, nnz=None, check=None):
+        """The matrix of a ``gsp_*`` count / fill pair: how every CSR whose number of entries
+        depends on the data is built.
+
+        ``count(stream, indptr, total)`` writes indptr (shape[0] + 1) and the int64 number of
+        entries to ``total``, a one-element device tensor, or to nothing when ``nnz`` is given
+        (``total`` is None then).  The total is read once; ``ValueError`` naming ``what`` when it
+        is 2^31 or more, where indptr has wrapped, and whatever ``check(nnz)`` raises, both
+        before indices and data are allocated.  ``fill(stream, indptr, indices, data)`` writes
+        the entries, ``dtype`` values on ``device``."""
+        torch = nat.require_cuda()
+        with torch.cuda.device(device):
+            st = nat.stream_ptr(device)
+            indptr = torch.empty(shape[0] + 1, dtype=torch.int32, device=device)
+            total = torch.empty(1, dtype=torch.int64, device=device)
+            count(st, indptr, None if nnz is not None else total)
+            if nnz is None:
+                nnz = int(total.item())
+            if nnz >= 2 ** 31:
+                raise ValueError("The {} would have {} entries; at most 2^31 - 1 are "
+                                 "supported.".format(what, nnz))
+            if check is not None:
+                check(nnz)
+            indices = torch.empty(nnz, dtype=torch.int32, device=device)
+            data = torch.empty(nnz, dtype=dtype, device=device)
+            fill(st, indptr, indices, data)
+        return cls(indptr, indices, data, shape)
+
     def _call(self, name, *args):
         """Native entry point ``name`` on this matrix's device and its current stream."""
         torch = nat.require_cuda()
@@ -201,26 +232,27 @@ class DeviceCSR:
             name, mode = "gsp_csr_symmetrize_", (nat.i32(_SYMMETRIZE_MODES[method]),)
         else:
             raise ValueError("Unknown symmetrization method {}.".format(method))
-        torch = nat.require_cuda()
         n, sfx = self.shape[0], nat.suffix(self.dtype)
         T = self.transpose() if transpose is None else transpose
         operands = (self.indptr, self.indices, self.data, T.indptr, T.indices, T.data)
-        sp = torch.empty(n + 1, dtype=torch.int32, device=self.device)
-        self._call(name + "count_" + sfx, nat.i64(n), *mode, *operands, sp)
-        si, sd = self._empty(int(sp[-1].item()) if n else 0)
-        self._call(name + "fill_" + sfx, nat.i64(n), *mode, *operands, sp, si, sd)
-        return DeviceCSR(sp, si, sd, self.shape)
+        return DeviceCSR.from_counts(
+            self.shape, self.dtype, self.device,
+            lambda st, sp, nnz: nat.call(name + "count_" + sfx, nat.i64(n), *mode, *operands, sp,
+                                         nnz, st),
+            lambda st, sp, si, sd: nat.call(name + "fill_" + sfx, nat.i64(n), *mode, *operands,
+                                            sp, si, sd, st),
+            "symmetrized matrix")
 
     def eliminate_zeros(self):
         """M without its stored zeros (graph.py:128), by the compaction kernels."""
-        torch = nat.require_cuda()
         n, sfx = self.shape[0], nat.suffix(self.dtype)
-        indptr = torch.empty(n + 1, dtype=torch.int32, device=self.device)
-        self._call("gsp_csr_compact_count_" + sfx, nat.i64(n), self.indptr, self.data, indptr)
-        indices, data = self._empty(int(indptr[-1].item()) if n else 0)
-        self._call("gsp_csr_compact_fill_" + sfx, nat.i64(n), self.indptr, self.indices, self.data,
-                   indptr, indices, data)
-        return DeviceCSR(indptr, indices, data, self.shape)
+        return DeviceCSR.from_counts(
+            self.shape, self.dtype, self.device,
+            lambda st, ip, nnz: nat.call("gsp_csr_compact_count_" + sfx, nat.i64(n), self.indptr,
+                                         self.data, ip, nnz, st),
+            lambda st, ip, ix, d: nat.call("gsp_csr_compact_fill_" + sfx, nat.i64(n), self.indptr,
+                                           self.indices, self.data, ip, ix, d, st),
+            "matrix")
 
     def induced(self, v, labels=None, increasing=False):
         """Entries of M[v, :][:, v] (m x m) for device int32 ids v, by map -> count -> fill.
@@ -239,21 +271,19 @@ class DeviceCSR:
             return S, None if increasing else S.indices
         mptr = torch.empty(n + 1, dtype=torch.int32, device=dev)
         mpos = torch.empty(m, dtype=torch.int32, device=dev)
-        s_indptr = torch.empty(m + 1, dtype=torch.int32, device=dev)
-        nnz = torch.empty(1, dtype=torch.int64, device=dev)
         self._call("gsp_vertex_map", nat.i64(n), nat.i64(m), v, mptr, mpos)
-        self._call("gsp_subgraph_count", nat.i64(m), self.indptr, self.indices, v, mptr, labels,
-                   s_indptr, nnz)
-        nnz = int(nnz.item())
-        if nnz >= 2 ** 31:
-            raise ValueError("The subgraph would have {} entries; at most 2^31 - 1 are "
-                             "supported.".format(nnz))
-        s_indices, s_data = self._empty(nnz)
-        rows = None if increasing else torch.empty(nnz, dtype=torch.int32, device=dev)
-        self._call("gsp_subgraph_fill_" + nat.suffix(self.dtype), nat.i64(m), self.indptr,
-                   self.indices, self.data, v, mptr, mpos, labels, s_indptr, s_indices, s_data,
-                   rows)
-        return DeviceCSR(s_indptr, s_indices, s_data, (m, m)), rows
+        rows = []
+
+        def fill(st, sp, si, sd):
+            rows.append(None if increasing else torch.empty_like(si))
+            nat.call("gsp_subgraph_fill_" + nat.suffix(self.dtype), nat.i64(m), self.indptr,
+                     self.indices, self.data, v, mptr, mpos, labels, sp, si, sd, rows[0], st)
+        S = DeviceCSR.from_counts(
+            (m, m), self.dtype, dev,
+            lambda st, sp, nnz: nat.call("gsp_subgraph_count", nat.i64(m), self.indptr,
+                                         self.indices, v, mptr, labels, sp, nnz, st),
+            fill, "subgraph")
+        return S, rows[0]
 
     # -- introspection --------------------------------------------------------
     @property

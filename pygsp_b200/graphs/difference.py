@@ -97,18 +97,15 @@ class DifferenceMixIn:
         self._call("gsp_incidence_t_fill", nat.i64(ne), sources, targets, weights, dw, lap,
                    nat.i32(directed), dt_indptr, dt_indices, dt_data)
 
-        d_indptr = torch.empty(n + 1, dtype=torch.int32, device=self.device)
-        with torch.cuda.device(self.device):
-            nat.call("gsp_incidence_count", nat.i64(n), W.indptr, W.indices,
-                     Wt.indptr if directed else None, Wt.indices if directed else None,
-                     d_indptr, self._stream())
-        d_indices = torch.empty(nnz, dtype=torch.int32, device=self.device)
-        d_data = torch.empty(nnz, dtype=self.dtype, device=self.device)
-        self._call("gsp_incidence_fill", nat.i64(n), lap, W.indptr, W.indices, W.data, eptr,
-                   Wt.indptr if directed else None, Wt.indices if directed else None,
-                   Wt.data if directed else None, dw, d_indptr, d_indices, d_data)
-
-        D = DeviceCSR(d_indptr, d_indices, d_data, (n, ne))
+        t = (Wt.indptr, Wt.indices, Wt.data) if directed else (None, None, None)
+        D = DeviceCSR.from_counts(
+            (n, ne), self.dtype, self.device,
+            lambda st, ip, total: nat.call("gsp_incidence_count", nat.i64(n), W.indptr, W.indices,
+                                           *t[:2], ip, total, st),
+            lambda st, ip, ix, d: nat.call("gsp_incidence_fill_" + self._sfx, nat.i64(n), lap,
+                                           W.indptr, W.indices, W.data, eptr, *t, dw, ip, ix, d,
+                                           st),
+            "differential operator", nnz=nnz)
         D.T = DeviceCSR(dt_indptr, dt_indices, dt_data, (ne, n))
         self._D = D
 

@@ -112,16 +112,12 @@ def grid2d_adjacency_device(N1, N2, dtype=None, device=None):
     """Grid2d adjacency built by ``gsp_grid2d_*`` (no host matrix)."""
     torch = nat.require_cuda()
     dev, dt = _device_of(device), _torch_dtype(torch, dtype)
-    n = N1 * N2
-    indptr = torch.empty(n + 1, dtype=torch.int32, device=dev)
-    with torch.cuda.device(dev):
-        nat.call("gsp_grid2d_count", nat.i64(N1), nat.i64(N2), indptr, nat.stream_ptr(dev))
-        nnz = int(indptr[-1].item())
-        indices = torch.empty(nnz, dtype=torch.int32, device=dev)
-        data = torch.empty(nnz, dtype=dt, device=dev)
-        nat.call("gsp_grid2d_fill_" + nat.suffix(dt), nat.i64(N1), nat.i64(N2), indptr, indices,
-                 data, nat.stream_ptr(dev))
-    return DeviceCSR(indptr, indices, data, (n, n))
+    shape = (nat.i64(N1), nat.i64(N2))
+    return DeviceCSR.from_counts(
+        (N1 * N2, N1 * N2), dt, dev,
+        lambda st, ip, nnz: nat.call("gsp_grid2d_count", *shape, ip, nnz, st),
+        lambda st, ip, ix, d: nat.call("gsp_grid2d_fill_" + nat.suffix(dt), *shape, ip, ix, d, st),
+        "graph")
 
 
 def _device_points(points, dev):
@@ -260,24 +256,18 @@ def radius_device(points, epsilon, p=2, device=None):
     pts = _device_points(points, dev)
     _require_finite(pts)
     n, dim = pts.shape
-    indptr = torch.empty(n + 1, dtype=torch.int32, device=dev)
-    total = torch.zeros(1, dtype=torch.int64, device=dev)
-    with torch.cuda.device(dev):
-        nat.call("gsp_radius_count", nat.i64(n), nat.i32(dim), pts, nat.f64(epsilon), nat.f64(p),
-                 indptr, total, nat.stream_ptr(dev))
-        nnz = int(total.item())
-        if nnz >= 2 ** 31:
-            raise ValueError("the radius graph has %d entries: more than int32 CSR offsets hold "
-                             "(lower epsilon)" % nnz)
+    cloud = (nat.i64(n), nat.i32(dim), pts, nat.f64(epsilon), nat.f64(p))
+
+    def fits_in_memory(nnz):
         free = torch.cuda.mem_get_info(dev)[0]
         if 12 * nnz > free:
             raise ValueError("the radius graph has %d entries (%d bytes): more than the free "
                              "device memory (%d bytes)" % (nnz, 12 * nnz, free))
-        indices = torch.empty(nnz, dtype=torch.int32, device=dev)
-        dist = torch.empty(nnz, dtype=torch.float64, device=dev)
-        nat.call("gsp_radius_fill_f64", nat.i64(n), nat.i32(dim), pts, nat.f64(epsilon),
-                 nat.f64(p), indptr, indices, dist, nat.stream_ptr(dev))
-    return DeviceCSR(indptr, indices, dist, (n, n))
+    return DeviceCSR.from_counts(
+        (n, n), torch.float64, dev,
+        lambda st, ip, nnz: nat.call("gsp_radius_count", *cloud, ip, nnz, st),
+        lambda st, ip, ix, d: nat.call("gsp_radius_fill_f64", *cloud, ip, ix, d, st),
+        "radius graph", check=fits_in_memory)
 
 
 def _gauss_weights_device(D, sigma, dt):

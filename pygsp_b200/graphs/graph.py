@@ -256,18 +256,15 @@ class Graph(FourierMixIn, DifferenceMixIn, ConnectivityMixIn, LayoutMixIn):
             self._D = None
         self.lap_type = lap_type
 
-        torch = nat.require_cuda()
         Ws, n = self._symmetric_adjacency(), self.n_vertices
         dw = self._degrees()[0]
-        lp = torch.empty(n + 1, dtype=torch.int32, device=self.device)
-        self._call("gsp_laplacian_count", nat.i64(n), Ws.indptr, Ws.indices, Ws.data, dw,
-                   nat.i32(_LAP[lap_type]), lp)
-        nnz = int(lp[-1].item()) if n else 0
-        li = torch.empty(nnz, dtype=torch.int32, device=self.device)
-        ld = torch.empty(nnz, dtype=self.dtype, device=self.device)
-        self._call("gsp_laplacian_fill", nat.i64(n), Ws.indptr, Ws.indices, Ws.data, dw,
-                   nat.i32(_LAP[lap_type]), lp, li, ld)
-        self.L = DeviceCSR(lp, li, ld, (n, n))
+        args = (nat.i64(n), Ws.indptr, Ws.indices, Ws.data, dw, nat.i32(_LAP[lap_type]))
+        self.L = DeviceCSR.from_counts(
+            (n, n), self.dtype, self.device,
+            lambda st, lp, nnz: nat.call("gsp_laplacian_count_" + self._sfx, *args, lp, nnz, st),
+            lambda st, lp, li, ld: nat.call("gsp_laplacian_fill_" + self._sfx, *args, lp, li, ld,
+                                            st),
+            "Laplacian")
 
     def _check_signal(self, s):
         r"""Validate a signal's first dimension (graph.py:632-640)."""

@@ -32,29 +32,16 @@ def _check_nnz(nnz):
                          "supported.".format(nnz))
 
 
-def _closed_form(count, fill, n, kwargs):
-    """DeviceCSR (n x n) of a count / fill pair of ``gsp_*`` entry points.  ``count(stream,
-    indptr)`` and ``fill(suffix, stream, indptr, indices, data)`` make the calls."""
-    torch = nat.require_cuda()
-    dev, dt = _device_of(kwargs.get("device")), _torch_dtype(torch, kwargs.get("dtype"))
-    indptr = torch.empty(n + 1, dtype=torch.int32, device=dev)
-    with torch.cuda.device(dev):
-        count(nat.stream_ptr(dev), indptr)
-        nnz = int(indptr[-1].item())
-        indices = torch.empty(nnz, dtype=torch.int32, device=dev)
-        data = torch.empty(nnz, dtype=dt, device=dev)
-        fill(nat.suffix(dt), nat.stream_ptr(dev), indptr, indices, data)
-    return DeviceCSR(indptr, indices, data, (n, n))
-
-
 def comet_adjacency_device(N, k, directed=False, dtype=None, device=None):
     """Adjacency of ``Comet(N, k)`` (k = 0: ``Path(N, directed)``) by ``gsp_comet_*``."""
     _check_nnz((N - 1) * (1 if directed else 2))
+    dt = _torch_dtype(nat.require_cuda(), dtype)
     args = (nat.i64(N), nat.i64(k), nat.i32(directed))
-    return _closed_form(
-        lambda st, ip: nat.call("gsp_comet_count", *args, ip, st),
-        lambda sfx, st, ip, ix, d: nat.call("gsp_comet_fill_" + sfx, *args, ip, ix, d, st),
-        N, dict(dtype=dtype, device=device))
+    return DeviceCSR.from_counts(
+        (N, N), dt, _device_of(device),
+        lambda st, ip, nnz: nat.call("gsp_comet_count", *args, ip, nnz, st),
+        lambda st, ip, ix, d: nat.call("gsp_comet_fill_" + nat.suffix(dt), *args, ip, ix, d, st),
+        "graph")
 
 
 class Path(Graph):
@@ -125,11 +112,14 @@ class Torus(Graph):
             raise ValueError("Nv and Mv must be positive.")
         row0 = {1 % Nv, (Nv - 1) % Nv, (1 % Mv) * Nv, ((Mv - 1) % Mv) * Nv}
         _check_nnz(Nv * Mv * len(row0))          # every row has as many entries as row 0
+        dt = _torch_dtype(nat.require_cuda(), kwargs.get("dtype"))
         args = (nat.i64(Nv), nat.i64(Mv))
-        W = _closed_form(
-            lambda st, ip: nat.call("gsp_torus_count", *args, ip, st),
-            lambda sfx, st, ip, ix, d: nat.call("gsp_torus_fill_" + sfx, *args, ip, ix, d, st),
-            Nv * Mv, kwargs)
+        W = DeviceCSR.from_counts(
+            (Nv * Mv, Nv * Mv), dt, _device_of(kwargs.get("device")),
+            lambda st, ip, nnz: nat.call("gsp_torus_count", *args, ip, nnz, st),
+            lambda st, ip, ix, d: nat.call("gsp_torus_fill_" + nat.suffix(dt), *args, ip, ix, d,
+                                           st),
+            "graph")
         phi = np.arange(Mv) * 2 * np.pi / Mv
         theta = np.arange(Nv) * 2 * np.pi / Nv
         radius = 1.5 + np.sin(phi)
@@ -152,11 +142,13 @@ class FullConnected(Graph):
         if N < 0:
             raise ValueError("negative dimensions are not allowed")
         _check_nnz(N * (N - 1))
-        W = _closed_form(
-            lambda st, ip: nat.call("gsp_full_connected_indptr", nat.i64(N), ip, st),
-            lambda sfx, st, ip, ix, d: nat.call("gsp_full_connected_fill_" + sfx, nat.i64(N),
-                                                ix, d, st),
-            N, kwargs)
+        dt = _torch_dtype(nat.require_cuda(), kwargs.get("dtype"))
+        W = DeviceCSR.from_counts(
+            (N, N), dt, _device_of(kwargs.get("device")),
+            lambda st, ip, nnz: nat.call("gsp_full_connected_indptr", nat.i64(N), ip, nnz, st),
+            lambda st, ip, ix, d: nat.call("gsp_full_connected_fill_" + nat.suffix(dt),
+                                           nat.i64(N), ix, d, st),
+            "graph")
         plotting = {"limits": np.array([-1, 1, -1, 1])}
         super().__init__(W, plotting=plotting, **kwargs)
 
@@ -227,13 +219,14 @@ class RandomRing(Graph):
         width = 2 * np.pi / N
         assert (gaps[gaps != 0].mean() - width) < 1e-10
         torch = nat.require_cuda()
-        dev = _device_of(kwargs.get("device"))
+        dev, dt = _device_of(kwargs.get("device")), _torch_dtype(torch, kwargs.get("dtype"))
         a_dev = torch.from_numpy(np.ascontiguousarray(a)).to(dev)
-        W = _closed_form(
-            lambda st, ip: nat.call("gsp_random_ring_count", nat.i64(N), a_dev, ip, st),
-            lambda sfx, st, ip, ix, d: nat.call("gsp_random_ring_fill_" + sfx, nat.i64(N), a_dev,
-                                                nat.f64(width), ip, ix, d, st),
-            N, kwargs)
+        W = DeviceCSR.from_counts(
+            (N, N), dt, dev,
+            lambda st, ip, nnz: nat.call("gsp_random_ring_count", nat.i64(N), a_dev, ip, nnz, st),
+            lambda st, ip, ix, d: nat.call("gsp_random_ring_fill_" + nat.suffix(dt), nat.i64(N),
+                                           a_dev, nat.f64(width), ip, ix, d, st),
+            "graph")
         coords = np.stack([np.cos(angles), np.sin(angles)], axis=1)
         plotting = {"limits": np.array([-1, 1, -1, 1])}
         super().__init__(W, coords=coords, plotting=plotting, **kwargs)
@@ -247,26 +240,19 @@ def line_graph_adjacency(graph, dtype=None):
 
     Calls ``graph.compute_differential_operator()``.  ``ValueError`` when the line graph would
     hold 2^31 entries or more, raised after the count and before anything else is allocated."""
-    torch = nat.require_cuda()
-    dt = _torch_dtype(torch, graph.dtype if dtype is None else dtype)
+    dt = _torch_dtype(nat.require_cuda(), graph.dtype if dtype is None else dtype)
     graph.compute_differential_operator()
-    D, W, ne, dev = graph.D, graph.W, graph.n_edges, graph.device
+    D, W, ne = graph.D, graph.W, graph.n_edges
     _, sources, targets, _, _ = graph._edges_device()
-    directed = nat.i32(graph.is_directed())
-    lg_indptr = torch.empty(ne + 1, dtype=torch.int32, device=dev)
-    nnz = torch.empty(1, dtype=torch.int64, device=dev)
-    operands = (sources, targets, D.indptr)
-    with torch.cuda.device(dev):
-        st = nat.stream_ptr(dev)
-        nat.call("gsp_line_graph_count", nat.i64(ne), *operands, W.indptr, W.indices, directed,
-                 lg_indptr, nnz, st)
-        total = int(nnz.item())
-        _check_nnz(total)
-        indices = torch.empty(total, dtype=torch.int32, device=dev)
-        data = torch.empty(total, dtype=dt, device=dev)
-        nat.call("gsp_line_graph_fill_" + nat.suffix(dt), nat.i64(ne), *operands, D.indices,
-                 W.indptr, W.indices, directed, lg_indptr, indices, data, st)
-    return DeviceCSR(lg_indptr, indices, data, (ne, ne)), sources, targets
+    head = (nat.i64(ne), sources, targets, D.indptr)
+    tail = (W.indptr, W.indices, nat.i32(graph.is_directed()))
+    A = DeviceCSR.from_counts(
+        (ne, ne), dt, graph.device,
+        lambda st, ip, nnz: nat.call("gsp_line_graph_count", *head, *tail, ip, nnz, st),
+        lambda st, ip, ix, d: nat.call("gsp_line_graph_fill_" + nat.suffix(dt), *head, D.indices,
+                                       *tail, ip, ix, d, st),
+        "line graph")
+    return A, sources, targets
 
 
 class LineGraph(Graph):

@@ -8,7 +8,9 @@ import pytest
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 
-def test_library_exports_every_declared_symbol():
+def test_library_exports_every_declared_symbol_at_abi_3():
+    """ABI 3: every CSR count entry point reports its int64 number of entries through a trailing
+    `int64_t* nnz`."""
     from pygsp_b200 import _native
     lib = _native.lib()
     names = _native.header_symbols()
@@ -18,7 +20,7 @@ def test_library_exports_every_declared_symbol():
         assert required in names
     missing = [n for n in names if not hasattr(lib, n)]
     assert not missing, missing
-    assert lib.gsp_abi_version() == 2
+    assert lib.gsp_abi_version() == 3
 
 
 def test_fista_history_matches_header():

@@ -7,7 +7,8 @@ One JSON line per measurement (also appended to --out when given):
   line_graph : the line graph of the config-2 graph (Sensor-type k-NN, 1e6 vertices, k = 10,
                Morton order, float32): gsp_line_graph_count and gsp_line_graph_fill separately,
                and LineGraph(G) end to end (D, edge list, count, fill and the Graph checks);
-  torus      : the adjacency of Torus(10_000, 10_000) (count, scan, fill);
+  torus      : gsp_torus_count of Torus(10_000, 10_000) alone (row sizes, int64 total, scan), and
+               the whole adjacency (count, fill);
   full       : the adjacency of FullConnected(30_000) (indptr, fill).
 Times are milliseconds per call from CUDA events after warm-up calls.  Each is reported beside
 the time the bytes it stores would take at the H100 SXM data-sheet HBM bandwidth (3.35 TB/s):
@@ -68,7 +69,7 @@ def main():
         raise SystemExit("structured_probe needs a CUDA device")
     import pygsp_b200 as gsp
     from pygsp_b200 import _native as nat
-    from pygsp_b200.graphs import structured
+    from pygsp_b200.graphs.csr import DeviceCSR
     emit(dict(kind="card", card=card(), torch=torch.__version__), a.out)
 
     # ---- line graph of config 2: count and fill apart
@@ -100,23 +101,31 @@ def main():
     del G, D, W, s, t
 
     # ---- Torus(10_000, 10_000) and FullConnected(30_000) adjacencies
+    args = (nat.i64(10_000), nat.i64(10_000))
+    indptr = torch.empty(10 ** 8 + 1, dtype=torch.int32, device=dev)
+
+    def torus_count():
+        nat.call("gsp_torus_count", *args, indptr, nnz, st)
+    ms = timed(torus_count, a.reps)
+    record("torus_count", ms, 4 * (10 ** 8 + 1), a.out, n=10 ** 8, nnz=int(nnz.item()))
+    del indptr
+
     def torus():
-        args = (nat.i64(10_000), nat.i64(10_000))
-        return structured._closed_form(
-            lambda st, ip: nat.call("gsp_torus_count", *args, ip, st),
-            lambda sfx, st, ip, ix, d: nat.call("gsp_torus_fill_" + sfx, *args, ip, ix, d, st),
-            10 ** 8, {})
+        return DeviceCSR.from_counts(
+            (10 ** 8, 10 ** 8), torch.float32, dev,
+            lambda st, ip, total: nat.call("gsp_torus_count", *args, ip, total, st),
+            lambda st, ip, ix, d: nat.call("gsp_torus_fill_f32", *args, ip, ix, d, st), "graph")
     ms = timed(torus, a.reps)
     record("torus", ms, 4 * (10 ** 8 + 1) + 8 * 4 * 10 ** 8, a.out, n=10 ** 8, nnz=4 * 10 ** 8)
 
     n = 30_000
 
     def full():
-        return structured._closed_form(
-            lambda st, ip: nat.call("gsp_full_connected_indptr", nat.i64(n), ip, st),
-            lambda sfx, st, ip, ix, d: nat.call("gsp_full_connected_fill_" + sfx, nat.i64(n),
-                                                ix, d, st),
-            n, {})
+        return DeviceCSR.from_counts(
+            (n, n), torch.float32, dev,
+            lambda st, ip, total: nat.call("gsp_full_connected_indptr", nat.i64(n), ip, total, st),
+            lambda st, ip, ix, d: nat.call("gsp_full_connected_fill_f32", nat.i64(n), ix, d, st),
+            "graph")
     ms = timed(full, a.reps)
     record("full", ms, 4 * (n + 1) + 8 * n * (n - 1), a.out, n=n, nnz=n * (n - 1))
 
