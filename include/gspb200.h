@@ -670,6 +670,23 @@ int gsp_radius_count(int64_t n, int d, const double* points, double epsilon, dou
                      int32_t* indptr, int64_t* nnz, void* stream);
 int gsp_radius_fill_f64(int64_t n, int d, const double* points, double epsilon, double p,
                         const int32_t* indptr, int32_t* indices, double* dist, void* stream);
+/* Segmented search: the vertices form n_seg contiguous segments, seg_start (n_seg + 1 int64,
+ * device) non-decreasing from 0 to n, and seg_id (n int32, device) the segment of every vertex
+ * (seg_start[seg_id[i]] <= i < seg_start[seg_id[i] + 1]).  Query i sees only the candidates of
+ * its own segment: the result is the unsegmented search of each segment alone, ids offset by
+ * the segment start, bit for bit.  The work is about the sum of the squared segment sizes.
+ * gsp_knn_brute_seg: 1 <= k <= 32; a vertex whose segment has fewer than k other points gets
+ *     its list padded with id -1 and distance 0. */
+int gsp_knn_brute_seg(int64_t n, int d, const double* points, int k, double p, int64_t n_seg,
+                      const int64_t* seg_start, const int32_t* seg_id, int32_t* nn_idx,
+                      double* nn_dist, void* stream);
+int gsp_radius_count_seg(int64_t n, int d, const double* points, double epsilon, double p,
+                         int64_t n_seg, const int64_t* seg_start, const int32_t* seg_id,
+                         int32_t* indptr, int64_t* nnz, void* stream);
+int gsp_radius_fill_seg_f64(int64_t n, int d, const double* points, double epsilon, double p,
+                            int64_t n_seg, const int64_t* seg_start, const int32_t* seg_id,
+                            const int32_t* indptr, int32_t* indices, double* dist,
+                            void* stream);
 
 #define GSPB200_DECLARE_NEIGHBOR_API(SUF, T)                                                     \
   int gsp_csr_symmetrize_count_##SUF(int64_t n, int mode, const int32_t* a_indptr,               \
@@ -917,6 +934,16 @@ int gsp_sparsify_sample(int64_t ne, const uint64_t* weights, int64_t q, uint64_t
  *   gsp_sbm_count writes offsets (n_chunks + 1): 0 then the inclusive scan of the entries each
  *   chunk emits.  gsp_sbm_fill writes the COO entries (vertex ids perm[position]) of chunk c at
  *   rows / cols [offsets[c], offsets[c + 1]).
+ * gsp_subset_select: a uniform n_s-subset of every pair space s, for Community's exact edge
+ *   counts.  The spaces are runs of consecutive plan rows, space s the chunks
+ *   [space_chunk_host[s], space_chunk_host[s + 1]) (host, n_spaces + 1, from 0 to n_chunks),
+ *   walked by gsp_sbm_count / gsp_sbm_fill with mirror 0, the identity perm and an inflated
+ *   probability into the candidates cand_rows / cand_cols (offsets: gsp_sbm_count's).  Each
+ *   candidate (u, v) gets the priority (x << 32) | y of the Philox block (u n + v, 2^63) of
+ *   `key`; the n_s = target_host[s] lowest (priority, candidate) of each space are kept and
+ *   written as (u, v), (v, u) to rows / cols, 2 sum(n_s) entries, space after space.  Synchronises
+ *   the stream once; -3 when a space has fewer than n_s candidates (redraw the walk with another
+ *   key) or when there are 2^31 candidates or more.
  * gsp_barabasi_albert: the attachment loop of barabasialbert.py:54-64.  Writes 2 m (n - m0)
  *   COO entries, (i, v) and (v, i) for each of the m targets v of each vertex i >= m0, in
  *   rounds of one launch each (the call synchronises the stream every few rounds);
@@ -928,6 +955,10 @@ int gsp_sbm_count(int64_t n_chunks, int64_t n_blocks, const int64_t* plan, const
 int gsp_sbm_fill(int64_t n_chunks, int64_t n_blocks, const int64_t* plan, const double* prob,
                  uint64_t key, const int32_t* perm, const int64_t* offsets, int32_t* rows,
                  int32_t* cols, int max_blocks, void* stream);
+int gsp_subset_select(int64_t n, int64_t n_chunks, const int64_t* offsets, int64_t n_spaces,
+                      const int64_t* space_chunk_host, const int64_t* target_host, uint64_t key,
+                      const int32_t* cand_rows, const int32_t* cand_cols, int32_t* rows,
+                      int32_t* cols, int max_blocks, void* stream);
 int gsp_barabasi_albert(int64_t n, int64_t m0, int64_t m, uint64_t key, int32_t* rows,
                         int32_t* cols, int max_blocks, int* rounds_host_out, void* stream);
 

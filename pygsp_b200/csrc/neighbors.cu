@@ -72,10 +72,16 @@ __device__ __forceinline__ void cp_wait() { asm volatile("cp.async.wait_group %0
 // MODE kKnn:   out_idx / out_dist are the (n, k) lists.
 // MODE kCount: indptr[i + 1] = row size.
 // MODE kFill:  row i is written at indptr[i] into out_idx / out_dist, in column order.
-template <int M, int MODE>
-__global__ void __launch_bounds__(kNbThreads, 2)
-    neighbors_kernel(int64_t n, int d, const double* __restrict__ pts, int k, double p,
-                     double eps_acc, int32_t* indptr, int32_t* out_idx, double* out_dist) {
+// SEG: query i only sees the candidates of its segment [seg_start[s], seg_start[s + 1]),
+// s = seg_id[i].  The CTA walks the candidate tiles covering the segments of its first and last
+// query only, and each query skips the columns of a tile outside its own segment -- the same
+// per-pair test, in the same (tile, column) order, as the unsegmented search of the segment.
+template <int M, int MODE, bool SEG>
+__device__ __forceinline__ void neighbors_body(int64_t n, int d, const double* __restrict__ pts,
+                                               int k, double p, double eps_acc, int32_t* indptr,
+                                               int32_t* out_idx, double* out_dist,
+                                               const int64_t* __restrict__ seg_start,
+                                               const int32_t* __restrict__ seg_id) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   double* sq = reinterpret_cast<double*>(smem_raw);   // [2][kQ][kLd]
   double* sc = sq + 2 * kQ * kLd;                     // [2][kC][kLd]
@@ -86,12 +92,25 @@ __global__ void __launch_bounds__(kNbThreads, 2)
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
   const int64_t q0 = int64_t(blockIdx.x) * kQ;
   const int nslab = (d + kS - 1) / kS;
-  const int64_t ntile = (n + kC - 1) / kC;
+  int64_t t0 = 0, ntile = (n + kC - 1) / kC;
+  int64_t seg_lo = 0, seg_hi = n;     // candidate range of this thread's query (SEG)
+  if (SEG) {
+    const int64_t qlast = (q0 + kQ < n ? q0 + kQ : n) - 1;
+    const int64_t c_lo = __ldg(seg_start + __ldg(seg_id + q0));
+    const int64_t c_hi = __ldg(seg_start + __ldg(seg_id + qlast) + 1);
+    t0 = c_lo / kC;
+    ntile = c_hi > c_lo ? (c_hi + kC - 1) / kC - t0 : 0;
+    if (tid < kQ && q0 + tid < n) {
+      const int s = __ldg(seg_id + q0 + tid);
+      seg_lo = __ldg(seg_start + s);
+      seg_hi = __ldg(seg_start + s + 1);
+    }
+  }
   const int64_t nstep = ntile * nslab;
 
   auto load = [&](int64_t step, int buf) {
-    const int64_t t = step / nslab;
-    const int dim0 = int(step - t * nslab) * kS;
+    const int64_t t = t0 + step / nslab;
+    const int dim0 = int(step - (t - t0) * nslab) * kS;
     double* dq = sq + buf * kQ * kLd;
     double* dc = sc + buf * kC * kLd;
     for (int e = tid; e < kQ * kS; e += kNbThreads) {
@@ -113,7 +132,7 @@ __global__ void __launch_bounds__(kNbThreads, 2)
   int64_t o = (MODE == kFill && selector) ? indptr[my_q] : 0;
 
   double acc[4][4];
-  load(0, 0);
+  if (!SEG || nstep > 0) load(0, 0);
   for (int64_t step = 0; step < nstep; ++step) {
     const int buf = int(step & 1);
     if (step + 1 < nstep) {
@@ -123,8 +142,8 @@ __global__ void __launch_bounds__(kNbThreads, 2)
       cp_wait<0>();
     }
     __syncthreads();
-    const int64_t t = step / nslab;
-    const int sl = int(step - t * nslab);
+    const int64_t t = t0 + step / nslab;
+    const int sl = int(step - (t - t0) * nslab);
     if (sl == 0) {
 #pragma unroll
       for (int i = 0; i < 4; ++i)
@@ -155,7 +174,12 @@ __global__ void __launch_bounds__(kNbThreads, 2)
         const int64_t c0 = t * kC;
         const int cn = n - c0 < kC ? int(n - c0) : kC;
         const double* row = sdist + tid * kDLd;
-        for (int c = 0; c < cn; ++c) {
+        int cb = 0, ce = cn;
+        if (SEG) {
+          cb = seg_lo > c0 ? int(seg_lo - c0 < kC ? seg_lo - c0 : kC) : 0;
+          ce = seg_hi - c0 < cn ? int(seg_hi - c0 > 0 ? seg_hi - c0 : 0) : cn;
+        }
+        for (int c = cb; c < ce; ++c) {
           const int64_t cand = c0 + c;
           if (cand == my_q) continue;
           const double a = row[c];
@@ -202,17 +226,45 @@ __global__ void __launch_bounds__(kNbThreads, 2)
   }
 }
 
+template <int M, int MODE>
+__global__ void __launch_bounds__(kNbThreads, 2)
+    neighbors_kernel(int64_t n, int d, const double* __restrict__ pts, int k, double p,
+                     double eps_acc, int32_t* indptr, int32_t* out_idx, double* out_dist) {
+  neighbors_body<M, MODE, false>(n, d, pts, k, p, eps_acc, indptr, out_idx, out_dist, nullptr,
+                                 nullptr);
+}
+
+template <int M, int MODE>
+__global__ void __launch_bounds__(kNbThreads, 2)
+    neighbors_seg_kernel(int64_t n, int d, const double* __restrict__ pts, int k, double p,
+                         double eps_acc, int32_t* indptr, int32_t* out_idx, double* out_dist,
+                         const int64_t* __restrict__ seg_start,
+                         const int32_t* __restrict__ seg_id) {
+  neighbors_body<M, MODE, true>(n, d, pts, k, p, eps_acc, indptr, out_idx, out_dist, seg_start,
+                                seg_id);
+}
+
+// seg_start == nullptr: the whole cloud; otherwise the segmented search (seg_id per vertex)
 template <int MODE>
 int launch_neighbors(int64_t n, int d, const double* pts, int k, double p, double eps_acc,
-                     int32_t* indptr, int32_t* out_idx, double* out_dist, cudaStream_t st) {
+                     int32_t* indptr, int32_t* out_idx, double* out_dist, cudaStream_t st,
+                     const int64_t* seg_start = nullptr, const int32_t* seg_id = nullptr) {
   const int blocks = (int)ceil_div(n, kQ);
 #define GSP_NB_LAUNCH(M)                                                                        \
   do {                                                                                          \
-    auto kern = neighbors_kernel<M, MODE>;                                                      \
-    GSP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,            \
-                                  (int)kSmemBytes));                                            \
-    kern<<<blocks, kNbThreads, kSmemBytes, st>>>(n, d, pts, k, p, eps_acc, indptr, out_idx,     \
-                                                 out_dist);                                     \
+    if (seg_start == nullptr) {                                                                 \
+      auto kern = neighbors_kernel<M, MODE>;                                                    \
+      GSP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,          \
+                                    (int)kSmemBytes));                                          \
+      kern<<<blocks, kNbThreads, kSmemBytes, st>>>(n, d, pts, k, p, eps_acc, indptr, out_idx,   \
+                                                   out_dist);                                   \
+    } else {                                                                                    \
+      auto kern = neighbors_seg_kernel<M, MODE>;                                                \
+      GSP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,          \
+                                    (int)kSmemBytes));                                          \
+      kern<<<blocks, kNbThreads, kSmemBytes, st>>>(n, d, pts, k, p, eps_acc, indptr, out_idx,   \
+                                                   out_dist, seg_start, seg_id);                \
+    }                                                                                           \
   } while (0)
   if (p == 1.0) GSP_NB_LAUNCH(kL1);
   else if (p == 2.0) GSP_NB_LAUNCH(kL2);
@@ -352,6 +404,45 @@ int gsp_radius_fill_f64(int64_t n, int d, const double* points, double epsilon, 
   return gsp::launch_neighbors<gsp::kFill>(n, d, points, 1, p, gsp::radius_key(epsilon, p),
                                            const_cast<int32_t*>(indptr), indices, dist,
                                            gsp::as_stream(stream));
+}
+
+#define GSP_REQUIRE_SEGMENTS(n_seg, seg_start, seg_id)                                         \
+  GSP_REQUIRE((n_seg) >= 1 && (seg_start) && (seg_id), "bad segment table")
+
+int gsp_knn_brute_seg(int64_t n, int d, const double* points, int k, double p, int64_t n_seg,
+                      const int64_t* seg_start, const int32_t* seg_id, int32_t* nn_idx,
+                      double* nn_dist, void* stream) {
+  GSP_REQUIRE_CLOUD(n, d, p);
+  GSP_REQUIRE_SEGMENTS(n_seg, seg_start, seg_id);
+  GSP_REQUIRE(k >= 1 && k <= gsp::kMaxNbK, "k must be in [1, 32]");
+  return gsp::launch_neighbors<gsp::kKnn>(n, d, points, k, p, 0.0, nullptr, nn_idx, nn_dist,
+                                          gsp::as_stream(stream), seg_start, seg_id);
+}
+
+int gsp_radius_count_seg(int64_t n, int d, const double* points, double epsilon, double p,
+                         int64_t n_seg, const int64_t* seg_start, const int32_t* seg_id,
+                         int32_t* indptr, int64_t* nnz, void* stream) {
+  GSP_REQUIRE_CLOUD(n, d, p);
+  GSP_REQUIRE_SEGMENTS(n_seg, seg_start, seg_id);
+  GSP_REQUIRE(epsilon >= 0, "epsilon must be >= 0");
+  cudaStream_t st = gsp::as_stream(stream);
+  const int rc = gsp::launch_neighbors<gsp::kCount>(n, d, points, 1, p,
+                                                    gsp::radius_key(epsilon, p), indptr, nullptr,
+                                                    nullptr, st, seg_start, seg_id);
+  if (rc != GSP_OK) return rc;
+  return gsp::scan_rows(indptr, n, nnz, st);
+}
+
+int gsp_radius_fill_seg_f64(int64_t n, int d, const double* points, double epsilon, double p,
+                            int64_t n_seg, const int64_t* seg_start, const int32_t* seg_id,
+                            const int32_t* indptr, int32_t* indices, double* dist,
+                            void* stream) {
+  GSP_REQUIRE_CLOUD(n, d, p);
+  GSP_REQUIRE_SEGMENTS(n_seg, seg_start, seg_id);
+  GSP_REQUIRE(epsilon >= 0, "epsilon must be >= 0");
+  return gsp::launch_neighbors<gsp::kFill>(n, d, points, 1, p, gsp::radius_key(epsilon, p),
+                                           const_cast<int32_t*>(indptr), indices, dist,
+                                           gsp::as_stream(stream), seg_start, seg_id);
 }
 
 #define GSP_NEIGHBOR_API(SUF, T)                                                                \

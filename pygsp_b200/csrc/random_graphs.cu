@@ -40,8 +40,19 @@
 // 32-bit volatile load is needed) and stops at a pointee that is not, until the next round.
 // No thread waits for another.  The lowest non-final slot always finalises, so the rounds end;
 // the host reads the pending count every kCheckEvery rounds and gives up after kMaxRounds.
+//
+// Exact-size subsets.  gsp_subset_select keeps a uniform n_s-subset of the candidate pairs the
+// SBM walk drew for each pair space s (a run of consecutive plan rows, walked with no mirror at
+// an inflated probability; the caller redraws when a space came up short).  Each candidate
+// (u, v) gets the 64-bit priority of the first two words of the Philox block (g, 2^63) of the
+// caller's key, g = u n + v its global pair index: one radix sort by priority, one stable radix
+// sort by space, and the first n_s of each space are kept, both orientations emitted.  Given
+// the walk's count k >= n_s, the walk's set is a uniform k-subset and the n_s lowest of k iid
+// priorities a uniform n_s-subset of it.  Ties (equal priorities) go to the earlier candidate.
 #include <cub/cub.cuh>
 #include <curand_kernel.h>
+
+#include <vector>
 
 #include "common.cuh"
 #include "gspb200.h"
@@ -220,6 +231,64 @@ __global__ void ba_emit_kernel(int64_t slots, int64_t m0, int64_t m,
   cols[2 * e + 1] = i;
 }
 
+// position of x among the n + 1 non-decreasing offsets: the last s < n with off[s] <= x
+__device__ __forceinline__ int64_t segment_of(const int64_t* __restrict__ off, int64_t n,
+                                              int64_t x) {
+  int64_t lo = 0, hi = n - 1;
+  while (lo < hi) {
+    const int64_t mid = (lo + hi + 1) >> 1;
+    if (__ldg(off + mid) <= x) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+
+__global__ void subset_begin_kernel(int64_t n_spaces, const int64_t* __restrict__ space_chunk,
+                                    const int64_t* __restrict__ offsets, int64_t* begin) {
+  const int64_t s = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (s <= n_spaces) begin[s] = __ldg(offsets + __ldg(space_chunk + s));
+}
+
+__global__ void __launch_bounds__(kThreads)
+subset_priority_kernel(int64_t n_cand, int64_t n, const int32_t* __restrict__ rows,
+                       const int32_t* __restrict__ cols, uint64_t key,
+                       unsigned long long* prio, int32_t* pos) {
+  for (int64_t e = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; e < n_cand;
+       e += int64_t(gridDim.x) * blockDim.x) {
+    const uint64_t g = uint64_t(__ldg(rows + e)) * uint64_t(n) + uint64_t(__ldg(cols + e));
+    curandStatePhilox4_32_10_t state;
+    curand_init(key, 1ull << 63, 4ull * g, &state);
+    const uint4 r4 = curand4(&state);
+    prio[e] = (uint64_t(r4.x) << 32) | r4.y;
+    pos[e] = (int32_t)e;
+  }
+}
+
+__global__ void __launch_bounds__(kThreads)
+subset_space_kernel(int64_t n_cand, int64_t n_spaces, const int64_t* __restrict__ begin,
+                    const int32_t* __restrict__ pos, int32_t* space) {
+  for (int64_t e = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; e < n_cand;
+       e += int64_t(gridDim.x) * blockDim.x)
+    space[e] = (int32_t)segment_of(begin, n_spaces, __ldg(pos + e));
+}
+
+// output pair o of space s is the (o - sel[s])-th candidate of s in (priority, position) order
+__global__ void __launch_bounds__(kThreads)
+subset_emit_kernel(int64_t total, int64_t n_spaces, const int64_t* __restrict__ sel,
+                   const int64_t* __restrict__ begin, const int32_t* __restrict__ order,
+                   const int32_t* __restrict__ cand_rows, const int32_t* __restrict__ cand_cols,
+                   int32_t* rows, int32_t* cols) {
+  for (int64_t o = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; o < total;
+       o += int64_t(gridDim.x) * blockDim.x) {
+    const int64_t s = segment_of(sel, n_spaces, o);
+    const int32_t e = __ldg(order + __ldg(begin + s) + (o - __ldg(sel + s)));
+    const int32_t u = __ldg(cand_rows + e), v = __ldg(cand_cols + e);
+    rows[2 * o] = u;
+    cols[2 * o] = v;
+    rows[2 * o + 1] = v;
+    cols[2 * o + 1] = u;
+  }
+}
+
 int grid_of(int64_t work, int max_blocks) {
   int64_t g = ceil_div(work, kThreads);
   if (max_blocks > 0 && g > max_blocks) g = max_blocks;
@@ -289,6 +358,80 @@ int barabasi_albert(int64_t n, int64_t m0, int64_t m, uint64_t key, int32_t* row
   return GSP_OK;
 }
 
+int subset_select(int64_t n, int64_t n_chunks, const int64_t* offsets, int64_t n_spaces,
+                  const int64_t* space_chunk_host, const int64_t* target_host, uint64_t key,
+                  const int32_t* cand_rows, const int32_t* cand_cols, int32_t* rows,
+                  int32_t* cols, int max_blocks, cudaStream_t st) {
+  for (int64_t s = 0; s < n_spaces; ++s)
+    if (space_chunk_host[s] > space_chunk_host[s + 1] || target_host[s] < 0)
+      return fail(GSP_ERR_ARG, "subset_select: %s", "bad space table");
+  if (space_chunk_host[0] != 0 || space_chunk_host[n_spaces] != n_chunks)
+    return fail(GSP_ERR_ARG, "subset_select: %s", "the spaces must cover the chunks");
+  std::vector<int64_t> begin(n_spaces + 1), sel(n_spaces + 1, 0);
+  Scratch<int64_t> tables(st);
+  GSP_CUDA(tables.alloc(3 * (n_spaces + 1)));
+  int64_t* d_chunk = tables.get();
+  int64_t* d_begin = d_chunk + (n_spaces + 1);
+  int64_t* d_sel = d_begin + (n_spaces + 1);
+  GSP_CUDA(cudaMemcpyAsync(d_chunk, space_chunk_host, sizeof(int64_t) * (n_spaces + 1),
+                           cudaMemcpyHostToDevice, st));
+  subset_begin_kernel<<<(unsigned)ceil_div(n_spaces + 1, kThreads), kThreads, 0, st>>>(
+      n_spaces, d_chunk, offsets, d_begin);
+  GSP_LAUNCH_CHECK("subset_begin");
+  GSP_CUDA(cudaMemcpyAsync(begin.data(), d_begin, sizeof(int64_t) * (n_spaces + 1),
+                           cudaMemcpyDeviceToHost, st));
+  GSP_CUDA(cudaStreamSynchronize(st));
+  for (int64_t s = 0; s < n_spaces; ++s) {
+    if (begin[s + 1] - begin[s] < target_host[s])
+      return fail(GSP_ERR_UNSUPPORTED, "subset_select: %s",
+                  "a pair space has fewer candidates than its target; redraw it");
+    sel[s + 1] = sel[s] + target_host[s];
+  }
+  const int64_t n_cand = begin[n_spaces], total = sel[n_spaces];
+  if (n_cand >= (int64_t(1) << 31))
+    return fail(GSP_ERR_UNSUPPORTED, "subset_select: %s", "2^31 candidates or more");
+  if (total == 0) return GSP_OK;
+  GSP_CUDA(cudaMemcpyAsync(d_sel, sel.data(), sizeof(int64_t) * (n_spaces + 1),
+                           cudaMemcpyHostToDevice, st));
+  Scratch<unsigned long long> prio(st);
+  Scratch<int32_t> idx(st);
+  GSP_CUDA(prio.alloc(2 * n_cand));
+  GSP_CUDA(idx.alloc(4 * n_cand));
+  unsigned long long* prio_in = prio.get();
+  unsigned long long* prio_out = prio_in + n_cand;
+  int32_t* pos_a = idx.get();
+  int32_t* pos_b = pos_a + n_cand;
+  int32_t* spc_in = pos_b + n_cand;
+  int32_t* spc_out = spc_in + n_cand;
+  const int grid = grid_of(n_cand, max_blocks);
+  const int items = (int)n_cand;
+  subset_priority_kernel<<<grid, kThreads, 0, st>>>(n_cand, n, cand_rows, cand_cols, key,
+                                                    prio_in, pos_a);
+  GSP_LAUNCH_CHECK("subset_priority");
+  int rc = cub_temp("cub::DeviceRadixSort::SortPairs", st, [&](void* tmp, size_t& bytes) {
+    return cub::DeviceRadixSort::SortPairs(tmp, bytes, prio_in, prio_out, pos_a, pos_b, items, 0,
+                                           64, st);
+  });
+  if (rc != GSP_OK) return rc;
+  const int32_t* order = pos_b;
+  if (n_spaces > 1) {                  // stable: each space keeps the priority order
+    int bits = 1;
+    while ((int64_t(1) << bits) < n_spaces) ++bits;
+    subset_space_kernel<<<grid, kThreads, 0, st>>>(n_cand, n_spaces, d_begin, pos_b, spc_in);
+    GSP_LAUNCH_CHECK("subset_space");
+    rc = cub_temp("cub::DeviceRadixSort::SortPairs", st, [&](void* tmp, size_t& bytes) {
+      return cub::DeviceRadixSort::SortPairs(tmp, bytes, spc_in, spc_out, pos_b, pos_a, items, 0,
+                                             bits, st);
+    });
+    if (rc != GSP_OK) return rc;
+    order = pos_a;
+  }
+  subset_emit_kernel<<<grid_of(total, max_blocks), kThreads, 0, st>>>(
+      total, n_spaces, d_sel, d_begin, order, cand_rows, cand_cols, rows, cols);
+  GSP_LAUNCH_CHECK("subset_emit");
+  return GSP_OK;
+}
+
 }  // namespace gsp
 
 // ------------------------------- C ABI ------------------------------------
@@ -309,6 +452,16 @@ int gsp_sbm_fill(int64_t n_chunks, int64_t n_blocks, const int64_t* plan, const 
               "empty plan");
   return gsp::sbm_fill(n_chunks, n_blocks, plan, prob, key, perm, offsets, rows, cols,
                        max_blocks, gsp::as_stream(stream));
+}
+int gsp_subset_select(int64_t n, int64_t n_chunks, const int64_t* offsets, int64_t n_spaces,
+                      const int64_t* space_chunk_host, const int64_t* target_host, uint64_t key,
+                      const int32_t* cand_rows, const int32_t* cand_cols, int32_t* rows,
+                      int32_t* cols, int max_blocks, void* stream) {
+  GSP_REQUIRE(n >= 1 && n < (int64_t(1) << 31) && n_chunks >= 0 && offsets, "bad arguments");
+  GSP_REQUIRE(n_spaces >= 1 && n_spaces < (int64_t(1) << 31) && space_chunk_host && target_host,
+              "bad space table");
+  return gsp::subset_select(n, n_chunks, offsets, n_spaces, space_chunk_host, target_host, key,
+                            cand_rows, cand_cols, rows, cols, max_blocks, gsp::as_stream(stream));
 }
 int gsp_barabasi_albert(int64_t n, int64_t m0, int64_t m, uint64_t key, int32_t* rows,
                         int32_t* cols, int max_blocks, int* rounds_host_out, void* stream) {

@@ -38,6 +38,34 @@ def compute_log_scales(lmin, lmax, Nscales, t1=1, t2=2):
     return np.exp(np.linspace(np.log(t2 / lmin), np.log(t1 / lmax), Nscales))
 
 
+def distanz(x, y=None):
+    r"""Euclidean distances between the columns of x and those of y (default x): the (cx, cy)
+    matrix sqrt|xx_i + yy_j - 2 x_i . y_j| of pygsp/utils.py, computed on the host by the same
+    Gram expansion.  A 1-D array is one row.  ``ValueError`` when x and y have different
+    numbers of rows."""
+    x = np.asarray(x)
+    if x.ndim < 2:
+        x = x.reshape(1, x.shape[0])
+    y = x if y is None else np.asarray(y)
+    if y.ndim < 2:
+        y = y.reshape(1, y.shape[0])
+    if x.shape[0] != y.shape[0]:
+        raise ValueError("The sizes of x and y do not fit")
+    xx = (x * x).sum(axis=0)
+    yy = (y * y).sum(axis=0)
+    xy = np.dot(x.T, y)
+    return np.sqrt(abs(xx[:, np.newaxis] + yy[np.newaxis, :] - 2 * xy))
+
+
+def rescale_center(x):
+    r"""Centre every row of x on its mean, then divide by the largest centred value
+    (pygsp/utils.py): ``rescale_center([[1, 6], [2, 5], [3, 4]])`` is
+    ``[[-1, 1], [-0.6, 0.6], [-0.2, 0.2]]``."""
+    x = np.asarray(x)
+    y = x - np.mean(x, axis=1)[:, np.newaxis]
+    return y / np.amax(y)
+
+
 def resistance_distance(G):
     r"""Resistance distances of a graph (pygsp/utils.py:140-181): a dense (N, N) float64 ndarray.
 
