@@ -962,6 +962,40 @@ int gsp_subset_select(int64_t n, int64_t n_chunks, const int64_t* offsets, int64
 int gsp_barabasi_albert(int64_t n, int64_t m0, int64_t m, uint64_t key, int32_t* rows,
                         int32_t* cols, int max_blocks, int* rounds_host_out, void* stream);
 
+/* ---------------------------------------------------------------- random regular ---
+ * gsp_random_regular: a simple undirected k-regular graph on n vertices (randomregular.py) by
+ *   stub pairing; n k even, 0 <= k < n (or k = 0), n k < 2^31, max_iter >= 1 attempts.  Every draw
+ *   is Philox4x32-10 of `key` at subsequence (attempt << 32) | phase (phase r: bulk round r;
+ *   GSPB200_RR_TAIL_STREAM, GSPB200_RR_SWITCH_STREAM) and an offset that is a pool position or a
+ *   draw number, so the graph depends on (key, n, k, max_iter) only, not on max_blocks (which caps
+ *   the grid; 0 = the default shape).  While the pool holds more than GSPB200_RR_TAIL_STUBS stubs,
+ *   rounds pair it after a stable sort by priority; one CTA finishes it by the reference's
+ *   sequential rule, restarting the attempt on a stuck pool (an exact check after
+ *   GSPB200_RR_CHECK_AFTER rejections in a row) or after GSPB200_RR_TAIL_DRAWS draws; the last
+ *   attempt places the remaining stubs by edge switches instead (at most GSPB200_RR_SWITCH_DRAWS
+ *   draws per stub pair, else the partial graph is kept).  Writes (u, v), (v, u) per edge to
+ *   rows / cols (room for n k entries); *entries_host_out gets their number (n k unless the graph
+ *   is partial), *attempts_host_out the attempts used, *rounds_host_out the rounds of all
+ *   attempts.  Synchronises the stream once per round and per attempt.  -3 if an attempt's rounds
+ *   do not reach the tail within GSPB200_RR_MAX_ROUNDS rounds.
+ * gsp_random_regular_complement: the complement (every j != i that is not a neighbour) of the
+ *   canonical CSR indptr / indices (n x n, symmetric, no loops), written as canonical CSR:
+ *   out_indptr (n + 1) and out_indices (nnz = n (n - 1) - indptr[n], given by the caller).
+ */
+#define GSPB200_RR_TAIL_STUBS 4096
+#define GSPB200_RR_CHECK_AFTER 32
+#define GSPB200_RR_TAIL_DRAWS (1 << 22)
+#define GSPB200_RR_SWITCH_DRAWS (1 << 16)
+#define GSPB200_RR_MAX_ROUNDS 4096
+#define GSPB200_RR_TAIL_STREAM 0xFFFFFFFFull
+#define GSPB200_RR_SWITCH_STREAM 0xFFFFFFFEull
+int gsp_random_regular(int64_t n, int64_t k, int max_iter, uint64_t key, int32_t* rows,
+                       int32_t* cols, int max_blocks, int* attempts_host_out,
+                       int* rounds_host_out, int64_t* entries_host_out, void* stream);
+int gsp_random_regular_complement(int64_t n, int64_t nnz, const int32_t* indptr,
+                                  const int32_t* indices, int32_t* out_indptr,
+                                  int32_t* out_indices, void* stream);
+
 /* ------------------------------------------------------------- structured graphs ---
  * The closed-form models of pygsp/graphs/{path,comet,star,torus,fullconnected,randomring}.py as
  * canonical CSR: each count writes indptr (n + 1) and the total, each fill the rows.

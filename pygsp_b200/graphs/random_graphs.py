@@ -1,7 +1,8 @@
-"""Random graph models sampled on the device (csrc/random_graphs.cu).
+"""Random graph models sampled on the device (csrc/random_graphs.cu, csrc/random_regular.cu).
 
-``ErdosRenyi`` and ``BarabasiAlbert`` (pygsp/graphs/erdosrenyi.py, barabasialbert.py) and the
-device sampler of ``StochasticBlockModel(backend='device')``.  The draws come from counter-based
+``ErdosRenyi``, ``BarabasiAlbert`` and ``RandomRegular`` (pygsp/graphs/erdosrenyi.py,
+barabasialbert.py, randomregular.py) and the device sampler of
+``StochasticBlockModel(backend='device')``.  The draws come from counter-based
 Philox streams keyed by a 64-bit key taken from ``np.random.default_rng(seed)``: a graph is a
 function of (seed, parameters) alone, whatever the launch shape, and a serial
 restatement of the samplers reproduces it bit for bit.  The streams are not the reference's,
@@ -22,6 +23,9 @@ from .graph import Graph, _torch_dtype
 _CHUNK_TARGET = 64
 # Grid cap of the sampling launches (0: the default shape).  Results do not depend on it.
 _MAX_BLOCKS = 0
+# Pool size below which one CTA finishes a random regular graph by the sequential rule
+# (GSPB200_RR_TAIL_STUBS of include/gspb200.h).  Part of the determinism contract.
+_TAIL_STUBS = 4096
 
 RECT, TRI_STRICT, TRI_LOOPS, OFF_DIAG = 0, 1, 2, 3
 PLAN_COLS = 8
@@ -167,3 +171,97 @@ class BarabasiAlbert(Graph):
 
     def _get_extra_repr(self):
         return dict(m0=self.m0, m=self.m, seed=self.seed)
+
+
+def random_regular_device(N, k, max_iter, key, dtype=None, device=None):
+    """(adjacency DeviceCSR, attempts, rounds) of one random k-regular graph drawn with Philox key
+    ``key`` (``gsp_random_regular``).  For k > (N - 1) / 2 the (N - 1 - k)-regular graph is drawn
+    and its complement written straight into CSR (``gsp_random_regular_complement``).  The
+    arguments must already be valid (see :class:`RandomRegular`)."""
+    torch = nat.require_cuda()
+    dev, dt = _device_of(device), _torch_dtype(torch, dtype)
+    kk = N - 1 - k if 2 * k > N - 1 else k
+    attempts, rounds, entries = ctypes.c_int(0), ctypes.c_int(0), ctypes.c_int64(0)
+    with torch.cuda.device(dev):
+        rows = torch.empty(N * kk, dtype=torch.int32, device=dev)
+        cols = torch.empty(N * kk, dtype=torch.int32, device=dev)
+        nat.call("gsp_random_regular", nat.i64(N), nat.i64(kk), nat.i32(max_iter), nat.u64(key),
+                 rows, cols, nat.i32(_MAX_BLOCKS), ctypes.byref(attempts), ctypes.byref(rounds),
+                 ctypes.byref(entries), nat.stream_ptr(dev))
+        m = entries.value
+        W = _assemble(rows[:m], cols[:m], N, dt)
+        if kk != k:
+            nnz = N * (N - 1) - W.nnz
+            if nnz >= 2 ** 31:
+                raise ValueError("The graph would have {} entries; at most 2^31 - 1 are "
+                                 "supported.".format(nnz))
+            indptr = torch.empty(N + 1, dtype=torch.int32, device=dev)
+            indices = torch.empty(nnz, dtype=torch.int32, device=dev)
+            nat.call("gsp_random_regular_complement", nat.i64(N), nat.i64(nnz), W.indptr,
+                     W.indices, indptr, indices, nat.stream_ptr(dev))
+            W = DeviceCSR(indptr, indices, torch.ones(nnz, dtype=dt, device=dev), (N, N))
+        return W, attempts.value, rounds.value
+
+
+class RandomRegular(Graph):
+    r"""Random k-regular graph (pygsp/graphs/randomregular.py): simple, undirected, unit weights,
+    every vertex adjacent to exactly k others.
+
+    Stub pairing on the device (``gsp_random_regular``): pairing rounds while more than
+    ``_TAIL_STUBS`` stubs are open, then the reference's sequential rule -- draw two open stubs,
+    keep the pair if it makes neither a loop nor a repeated edge -- with a restart when no legal
+    pair is left, up to ``max_iter`` attempts; the last attempt places its remaining stubs by edge
+    switches rather than giving up.  For k > (N - 1) / 2 the complement of an (N - 1 - k)-regular
+    graph is built.  The Philox key is ``np.random.default_rng(seed).integers(2**63)``.
+    ``_attempts`` and ``_rounds`` record the attempts and pairing rounds used.
+
+    ``ValueError`` when N k is odd (the reference's message), k < 0, k >= N (no such graph),
+    max_iter < 1 or N k >= 2^31, before anything is allocated on the device.
+    """
+
+    def __init__(self, N=64, k=6, max_iter=10, seed=None, **kwargs):
+        self.k = k
+        self.max_iter = max_iter
+        self.seed = seed
+        if (N * k) % 2 == 1:
+            raise ValueError("input error: N*d must be even!")
+        if k < 0:
+            raise ValueError("The degree k must be non-negative, got {}.".format(k))
+        if k >= max(N, 1):
+            raise ValueError("A {}-regular graph on {} vertices does not exist: k must be below "
+                             "N.".format(k, N))
+        if max_iter < 1:
+            raise ValueError("max_iter must be at least 1, got {}.".format(max_iter))
+        if N * k >= 2 ** 31:
+            raise ValueError("The graph would have {} entries; at most 2^31 - 1 are "
+                             "supported.".format(N * k))
+        key = int(np.random.default_rng(seed).integers(2 ** 63))
+        W, self._attempts, self._rounds = random_regular_device(
+            N, k, max_iter, key, kwargs.get("dtype"), kwargs.get("device"))
+        super().__init__(W, **kwargs)
+        self.is_regular()
+
+    def is_regular(self):
+        r"""Troubleshoot a given regular graph: log the reference's warning when the graph is not
+        symmetric, has parallel edges (a weight above 1), is not d-regular or has self-loops.
+        Computed on the device from ``is_directed()``, the weights, ``d`` and ``has_loops()``."""
+        warn = False
+        msg = "The given matrix"
+        if self.is_directed():
+            warn = True
+            msg = "{} is not symmetric,".format(msg)
+        if self.W.nnz and bool((self.W.data > 1).any()):
+            warn = True
+            msg = "{} has parallel edges,".format(msg)
+        d = self.d
+        if d.size and d.min() != d.max():
+            warn = True
+            msg = "{} is not d-regular,".format(msg)
+        if self.has_loops():
+            warn = True
+            msg = "{} has self loop.".format(msg)
+        if warn:
+            self.logger.warning("{}.".format(msg[:-1]))
+
+    def _get_extra_repr(self):
+        return dict(k=self.k, seed=self.seed)
