@@ -1048,6 +1048,49 @@ int gsp_line_graph_count(int64_t n_edges, const int32_t* sources, const int32_t*
 GSPB200_DECLARE_STRUCT_API(f32, float)
 GSPB200_DECLARE_STRUCT_API(f64, double)
 
+/* ------------------------------------------------------------ tree multiresolution ---
+ * pygsp/reduction.py: tree_multiresolution (pygsp_b200/reduction.py, csrc/tree.cu).  The tree is
+ * the canonical symmetric CSR indptr / indices / data (n x n, 1 <= n <= 2^30, nnz stored entries);
+ * diagonal entries are ignored.  Vertex ids are int32.
+ * gsp_tree_arc_count: arc_ptr (n + 1) := 0 and the inclusive scan of each row's off-diagonal
+ *   entries (the arcs, in CSR order); *n_arcs (device, int64) := their number.
+ * gsp_tree_root_*: depth, parent (int32, n) and wpar (double, n: the weight of the edge to the
+ *   parent, as stored, widened) of every vertex from `root`; depth[root] = 0, parent[root] = root,
+ *   wpar[root] = 0.  Needs a connected graph with n_arcs = 2 (n - 1) (a tree) and arc_ptr from
+ *   gsp_tree_arc_count.  Euler tour (twin by binary search, successor the next arc of the twin's
+ *   row) ranked by ceil(log2 n_arcs) rounds of pointer jumping, then a scan of +-1 over the tour:
+ *   O(log n) launches, no host synchronisation.
+ * gsp_tree_keep: new_id (n + 1) := 0 and the inclusive scan of (depth[v] even), i.e. new_id[v] is
+ *   v's id among the kept (even-depth) vertices; *n_new (device, int64) := their number.
+ * gsp_tree_coarsen_*: one level.  Every kept v (new id i) writes keep[i] = v (int64) and
+ *   new_depth[i] = depth[v] / 2; the root new_parent[i] = i, new_wpar[i] = 0; any other kept v, with
+ *   p = parent[v], g = parent[p] and j = new_id[g], new_parent[i] = j and the edge (i, j) of weight
+ *   c = (T) combine(wpar[v], wpar[p]), in double, for method GSPB200_TREE_UNWEIGHTED (1),
+ *   GSPB200_TREE_SUM (wv + wp) or GSPB200_TREE_RESISTANCE (1 / (1 / wv + 1 / wp)); new_wpar[i] = c
+ *   widened.  The edges are written as COO at rows / cols / vals [e] = (i, j, c) and [m + e] =
+ *   (j, i, c), m = n_new - 1, e the edge's place among the kept non-root vertices.
+ */
+#define GSPB200_TREE_UNWEIGHTED 0
+#define GSPB200_TREE_SUM 1
+#define GSPB200_TREE_RESISTANCE 2
+int gsp_tree_arc_count(int64_t n, const int32_t* indptr, const int32_t* indices, int32_t* arc_ptr,
+                       int64_t* n_arcs, void* stream);
+int gsp_tree_keep(int64_t n, const int32_t* depth, int32_t* new_id, int64_t* n_new,
+                  void* stream);
+
+#define GSPB200_DECLARE_TREE_API(SUF, T)                                                         \
+  int gsp_tree_root_##SUF(int64_t n, int64_t nnz, const int32_t* indptr, const int32_t* indices,  \
+                          const T* data, const int32_t* arc_ptr, int32_t root, int32_t* depth,   \
+                          int32_t* parent, double* wpar, void* stream);                          \
+  int gsp_tree_coarsen_##SUF(int64_t n, int64_t n_new, const int32_t* depth,                      \
+                             const int32_t* parent, const double* wpar, const int32_t* new_id,   \
+                             int32_t root, int method, int64_t* keep, int32_t* rows,             \
+                             int32_t* cols, T* vals, int32_t* new_depth, int32_t* new_parent,    \
+                             double* new_wpar, void* stream);
+
+GSPB200_DECLARE_TREE_API(f32, float)
+GSPB200_DECLARE_TREE_API(f64, double)
+
 #ifdef __cplusplus
 }
 #endif

@@ -8,7 +8,10 @@ The multiresolution sequence itself runs on the device too (DESIGN.md section 4.
 ``graph_multiresolution`` (largest-eigenvector down-sampling by Chebyshev-filtered subspace
 iteration), :func:`kron_reduction` (independent Schur blocks per component of the removed
 vertices, csrc/schur.cu) and :func:`graph_sparsify` (effective resistances from one float64
-factor, seeded Philox sampling).
+factor, seeded Philox sampling).  :func:`tree_multiresolution` (reduction.py:633-787, which
+cannot run in the reference) coarsens a tree to its even-depth vertices level after level: the
+tree is rooted by an Euler tour ranked by pointer jumping, in O(log N) launches whatever its depth,
+and each level is a few O(N) kernels (csrc/tree.cu, DESIGN.md section 4.21).
 
 A graph of the sequence carries ``G.mr = {'idx': kept vertices of the level above,
 'K_reg': ...}`` like the reference's.  Shapes: the reference keeps consistent shapes only for
@@ -416,6 +419,130 @@ def graph_multiresolution(G, levels, sparsify=True, sparsify_eps=None,
         Gs[i].mr["green_kernel"] = filters.Filter(Gs[i], lambda x: 1.0 / (reg_eps + x))
         Gs[i].mr["_green_eps"] = reg_eps
     return Gs
+
+
+_TREE_METHODS = {"unweighted": 0, "sum": 1, "resistance_distance": 2}   # GSPB200_TREE_*
+_TREE_MAX_N = 2 ** 30
+
+
+def _tree_root(G, root):
+    """(depth, parent, weight to parent) device tensors (int32, int32, float64) of the tree
+    ``G._symmetric_adjacency()`` rooted at ``root`` (csrc/tree.cu).  ``ValueError`` when the
+    graph is not connected or is not a tree."""
+    torch = nat.require_cuda()
+    n, dev = G.N, G.device
+    if n > _TREE_MAX_N:
+        raise ValueError("Tree multiresolution supports at most 2^30 vertices, not {}.".format(n))
+    if not 0 <= root < n:
+        raise ValueError("The root {} is not a vertex of the graph (N = {}).".format(root, n))
+    Ws = G._symmetric_adjacency()
+    with torch.cuda.device(dev):
+        st = nat.stream_ptr(dev)
+        # components of the symmetric adjacency: cc_labels reads the entries above the diagonal,
+        # which a directed W need not store
+        labels = torch.empty(n, dtype=torch.int32, device=dev)
+        ncomp = torch.empty(1, dtype=torch.int64, device=dev)
+        nat.call("gsp_cc_labels_" + G._sfx, nat.i64(n), Ws.indptr, Ws.indices, Ws.data, nat.i32(0),
+                 labels, ncomp, st)
+        arc_ptr = torch.empty(n + 1, dtype=torch.int32, device=dev)
+        n_arcs = torch.empty(1, dtype=torch.int64, device=dev)
+        nat.call("gsp_tree_arc_count", nat.i64(n), Ws.indptr, Ws.indices, arc_ptr, n_arcs, st)
+        counts = torch.cat([ncomp, n_arcs]).cpu().numpy()
+        if counts[0] != 1:
+            raise ValueError("Graph is not connected")
+        if counts[1] != 2 * (n - 1):
+            raise ValueError("G must be a tree: a connected graph on {} vertices with {} edges "
+                             "has {} off-diagonal entries, not {}.".format(
+                                 n, n - 1, int(counts[1]), 2 * (n - 1)))
+        depth = torch.empty(n, dtype=torch.int32, device=dev)
+        parent = torch.empty(n, dtype=torch.int32, device=dev)
+        wpar = torch.empty(n, dtype=torch.float64, device=dev)
+        nat.call("gsp_tree_root_" + G._sfx, nat.i64(n), nat.i64(Ws.nnz), Ws.indptr, Ws.indices,
+                 Ws.data, arc_ptr, nat.i32(root), depth, parent, wpar, st)
+    return depth, parent, wpar
+
+
+def _tree_depths(G, root):
+    """(depth, parent) of every vertex of the tree G from ``root``, as int32 device tensors."""
+    depth, parent, _ = _tree_root(G, int(root))
+    return depth, parent
+
+
+def _tree_level(G, depth, parent, wpar, root, method):
+    """One coarsening of a rooted tree: (keep (host int64), Graph of the kept vertices, new root,
+    and the next level's depth, parent and weight to parent)."""
+    from .graphs import Graph
+    torch = nat.require_cuda()
+    n, dev = int(depth.numel()), G.device
+    with torch.cuda.device(dev):
+        st = nat.stream_ptr(dev)
+        new_id = torch.empty(n + 1, dtype=torch.int32, device=dev)
+        n_new_dev = torch.empty(1, dtype=torch.int64, device=dev)
+        nat.call("gsp_tree_keep", nat.i64(n), depth, new_id, n_new_dev, st)
+        n_new = int(n_new_dev.item())
+        m = 2 * (n_new - 1)
+        keep = torch.empty(n_new, dtype=torch.int64, device=dev)
+        rows = torch.empty(m, dtype=torch.int32, device=dev)
+        cols = torch.empty(m, dtype=torch.int32, device=dev)
+        vals = torch.empty(m, dtype=G.dtype, device=dev)
+        new_depth = torch.empty(n_new, dtype=torch.int32, device=dev)
+        new_parent = torch.empty(n_new, dtype=torch.int32, device=dev)
+        new_wpar = torch.empty(n_new, dtype=torch.float64, device=dev)
+        nat.call("gsp_tree_coarsen_" + G._sfx, nat.i64(n), nat.i64(n_new), depth, parent, wpar,
+                 new_id, nat.i32(root), nat.i32(_TREE_METHODS[method]), keep, rows, cols, vals,
+                 new_depth, new_parent, new_wpar, st)
+        keep_host = keep.cpu().numpy()
+        new_root = int(np.searchsorted(keep_host, root))
+        W = DeviceCSR.from_coo(rows, cols, vals, (n_new, n_new))
+    Gn = Graph(W, lap_type=G.lap_type, coords=G.coords[keep_host] if hasattr(G, "coords") else None,
+               plotting=G.plotting, dtype=G.dtype, device=dev)
+    Gn.root = new_root
+    return keep_host, Gn, new_root, new_depth, new_parent, new_wpar
+
+
+def tree_multiresolution(G, Nlevel, reduction_method="resistance_distance",
+                         compute_full_eigen=False, root=None):
+    r"""Compute a multiresolution of trees (reduction.py:633-787).
+
+    ``G`` must be a tree: its symmetric adjacency (W, or (W + W^T) / 2 when directed; self-loops
+    ignored) is connected with 2 (N - 1) off-diagonal entries, else ``ValueError``.  ``root``:
+    ``G.root`` when None and G has one, else 1; an explicit 0 is honoured.  Per level, the
+    vertices of even depth are kept (in increasing order), and every kept vertex other than the
+    root is joined to its grandparent by an edge whose weight combines the weights w(v) to the
+    parent and w(p) from the parent to the grandparent: 1 (``'unweighted'``), w(v) + w(p)
+    (``'sum'``) or 1 / (1 / w(v) + 1 / w(p)) (``'resistance_distance'``), in float64, rounded once
+    to ``G.dtype``.  Depths are halved, the root keeps its place.
+
+    The tree is rooted on the device by an Euler tour ranked by pointer jumping, in O(log N)
+    launches whatever its depth, and each level is a few O(N) kernels (csrc/tree.cu; DESIGN.md
+    section 4.21).  Returns ``(Gs, subsampled_vertex_indices)``: ``Gs[0] is G`` and ``Nlevel``
+    coarser graphs (each with ``root``, the level's coordinates, ``lap_type`` and ``dtype`` of G,
+    and ``mr = {'idx', 'orig_idx', 'level'}`` as :func:`graph_multiresolution` sets, so
+    :func:`pyramid_analysis` and :func:`pyramid_synthesis` run on the pyramid), and the
+    ``Nlevel`` ascending int64 arrays of the kept vertices.  ``compute_full_eigen`` computes the
+    Fourier basis of every level, ``Gs[0]`` included.  A level of one vertex has no edge; the
+    levels after it repeat it.
+    """
+    if reduction_method not in _TREE_METHODS:
+        raise ValueError("Unknown graph reduction method.")
+    if root is None:
+        root = getattr(G, "root", 1)
+    root = int(root)
+    depth, parent, wpar = _tree_root(G, root)
+    if compute_full_eigen:
+        G.compute_fourier_basis()
+    Gs = [G]
+    G.mr = {"idx": np.arange(G.N), "orig_idx": np.arange(G.N)}
+    subsampled_vertex_indices = []
+    for lev in range(Nlevel):
+        keep, Gn, root, depth, parent, wpar = _tree_level(Gs[lev], depth, parent, wpar, root,
+                                                          reduction_method)
+        Gn.mr = {"idx": keep, "orig_idx": Gs[lev].mr["orig_idx"][keep], "level": lev}
+        if compute_full_eigen:
+            Gn.compute_fourier_basis()
+        Gs.append(Gn)
+        subsampled_vertex_indices.append(keep)
+    return Gs, subsampled_vertex_indices
 
 
 def _kron_regularized(G, ind, reg_eps):
