@@ -904,6 +904,22 @@ GSPB200_DECLARE_CONN_API(f64, double)
  *   sum(weights) (uint64 integer weights, sum < 2^64) picked e -- dist.rvs(size=q) and the
  *   removed stats.itemfreq of graph_sparsify (:104-115).  Draws come from Philox streams of
  *   `seed` (curand_kernel.h): the counts depend on (seed, weights, q) only.
+ * gsp_jl_sketch_f64, gsp_jl_accumulate_f64: the effective resistances of graph_sparsify (:84,
+ *   :101) without a dense factor, by the Johnson-Lindenstrauss sketch of Spielman-Srivastava
+ *   (csrc/resistance.cu).  L (n x n, canonical float64 CSR, non-positive off-diagonal entries:
+ *   only those are read, W = -offdiag(L)), dinv[i] = (W 1)[i]^-1/2 (0 for an isolated vertex),
+ *   k columns of which a call handles the block j0 .. j0 + width - 1 (1 <= width <= 256,
+ *   j0 + width <= k).
+ *   Philox convention: the sign of edge {a < b} in column j is +1 when bit (j mod 128) of the 128
+ *   bits of curand4 after curand_init(key, a n + b, 4 (j div 128)) is 0, else -1; bit t of the
+ *   128 is bit (t mod 32) of word (t div 32) of (x, y, z, w).
+ * gsp_jl_sketch_f64: Y (n x width, row-major, double) := column j - j0 of
+ *   D^-1/2 B^T W^1/2 q_j / sqrt(k): Y[i][j - j0] = dinv[i] / sqrt(k) * sum over the off-diagonal
+ *   entries (i, v) of row i, in CSR order, of s sqrt(-L_iv) q_j({i, v}), s = +1 when i > v, else
+ *   -1.  Every entry of Y is written.
+ * gsp_jl_accumulate_f64: R[e] += sum over the block's columns c, in order, of
+ *   (dinv[u] U[u][c] - dinv[v] U[v][c])^2 for u = erow[e], v = ecol[e] (ne edges), with U
+ *   (n x width, row-major) the solution of D^-1/2 (D - W) D^-1/2 U = Y, D = diag(W 1).
  */
 int gsp_schur_small_f64(const int32_t* indptr, const int32_t* indices, const double* data,
                         const int32_t* slot, const int32_t* cvert, const int32_t* cptr,
@@ -918,6 +934,11 @@ int gsp_edge_resistance_f64(int64_t ne, const int32_t* erow, const int32_t* ecol
                             const double* ainv, int64_t lda, double* R, void* stream);
 int gsp_sparsify_sample(int64_t ne, const uint64_t* weights, int64_t q, uint64_t seed,
                         int64_t* counts, void* stream);
+int gsp_jl_sketch_f64(int64_t n, const int32_t* indptr, const int32_t* indices, const double* data,
+                      const double* dinv, uint64_t key, int64_t j0, int64_t width, int64_t k,
+                      double* Y, void* stream);
+int gsp_jl_accumulate_f64(int64_t ne, const int32_t* erow, const int32_t* ecol, const double* U,
+                          const double* dinv, int64_t width, double* R, void* stream);
 
 /* ---------------------------------------------------------------- random graphs ---
  * Draws come from Philox4x32-10 streams of `key` (curand_kernel.h) whose subsequence is a chunk

@@ -126,8 +126,10 @@ def classification_tikhonov_simplex(G, y, M, tau=0.1, **kwargs):
     return X.cpu().numpy().astype(np.float64 if G.dtype == torch.float64 else np.float32)
 
 
-def _block_cg(G, tau, row_scale, diag, B, tol, maxiter):
-    """Solve (diag(row_scale) tau L + diag(diag)) X = B on the device; B (N, nsig) tensor."""
+def _block_cg(G, tau, row_scale, diag, B, tol, maxiter, patience=8):
+    """Solve (diag(row_scale) tau L + diag(diag)) X = B on the device; B (N, nsig) tensor.
+    Stops early when the worst residual has not halved over ``patience`` batches of 25
+    iterations."""
     torch = nat.require_cuda()
     L = G.L
     n, nsig = B.shape
@@ -153,7 +155,7 @@ def _block_cg(G, tau, row_scale, diag, B, tol, maxiter):
             best, stall = worst, 0
         else:
             stall += 1
-            if stall >= 8:
+            if stall >= patience:
                 break
     logger.warning("conjugate gradients stopped at relative residual %.2e after %d iterations",
                    worst, done)

@@ -8,7 +8,8 @@ The multiresolution sequence itself runs on the device too (DESIGN.md section 4.
 ``graph_multiresolution`` (largest-eigenvector down-sampling by Chebyshev-filtered subspace
 iteration), :func:`kron_reduction` (independent Schur blocks per component of the removed
 vertices, csrc/schur.cu) and :func:`graph_sparsify` (effective resistances from one float64
-factor, seeded Philox sampling).  :func:`tree_multiresolution` (reduction.py:633-787, which
+factor or, past its size, from a Johnson-Lindenstrauss sketch solved by block CG, csrc/resistance.cu
+and DESIGN.md section 4.22; seeded Philox sampling).  :func:`tree_multiresolution` (reduction.py:633-787, which
 cannot run in the reference) coarsens a tree to its even-depth vertices level after level: the
 tree is rooted by an Euler tour ranked by pointer jumping, in O(log N) launches whatever its depth,
 and each level is a few O(N) kernels (csrc/tree.cu, DESIGN.md section 4.21).
@@ -180,9 +181,9 @@ def _asymmetry(M):
     return int(count.item())
 
 
-def _check_symmetric(M):
+def _check_symmetric(M, what="Kron reduction"):
     if _asymmetry(M):
-        raise ValueError("Kron reduction on the device needs a symmetric matrix.")
+        raise ValueError("{} on the device needs a symmetric matrix.".format(what))
 
 
 def _kept_ids(ind, n):
@@ -297,7 +298,91 @@ def _sampling_seed(seed, i):
     return (int(0 if seed is None else seed) * 0x9E3779B97F4A7C15 + i) & 0xFFFFFFFFFFFFFFFF
 
 
-def graph_sparsify(M, epsilon, maxiter=10, seed=None):
+# The resistance sketch (DESIGN.md section 4.22): CG stops at this relative residual per column,
+# and its blocks of columns keep five (N, width) float64 arrays within this many bytes whatever
+# the card, so that (seed, k, N) gives the same bits on any card.
+_SKETCH_TOL = 1e-8
+_SKETCH_BYTES = 32 << 30
+_SKETCH_MAX_WIDTH = 256
+
+
+def _sketch_dim(n, delta=0.5):
+    """Default number of JL columns, ceil(24 ln N / delta^2) (at least 1)."""
+    return max(1, int(np.ceil(24 * np.log(max(n, 1)) / delta ** 2)))
+
+
+def _sketch_width(n, k):
+    """Columns per CG block: min(k, 256, w_mem), w_mem the largest power of two >= 8 with
+    5 * 8 * N * w_mem <= _SKETCH_BYTES; ValueError when even 8 columns do not fit."""
+    if 5 * 8 * n * 8 > _SKETCH_BYTES:
+        raise ValueError("The resistance sketch of this {0} x {0} Laplacian needs at least {1:.1f} "
+                         "GB of device memory for a block of 8 columns (at most {2:.1f} GB are "
+                         "used).".format(n, 5 * 8 * n * 8 / 2 ** 30, _SKETCH_BYTES / 2 ** 30))
+    w = 8
+    while w < _SKETCH_MAX_WIDTH and 5 * 8 * n * (2 * w) <= _SKETCH_BYTES:
+        w *= 2
+    return min(int(k), _SKETCH_MAX_WIDTH, w)
+
+
+def _sketch_maxiter(n):
+    """(CG iterations allowed per block, batches of 25 without halving the residual before CG
+    gives up): 20 sqrt(N), at least 1000, and sqrt(N) / 25, at least 8.  A two-dimensional mesh
+    of N vertices has a Jacobi-scaled condition number kappa that grows like N; CG needs about
+    sqrt(kappa) / 3 iterations to halve its residual and a multiple of sqrt(kappa) to reach
+    _SKETCH_TOL."""
+    return int(max(1000, 20 * np.sqrt(n))), int(max(8, np.sqrt(n) / 25))
+
+
+def _edge_resistances(Ld, start, end, k, seed):
+    """Effective resistances of the edges (start[e], end[e]) of the float64 Laplacian DeviceCSR
+    ``Ld`` by the Johnson-Lindenstrauss sketch with ``k`` columns (a float64 device tensor).
+
+    R~_e = ||Z (chi_u - chi_v)||^2, Z = Q W^1/2 B L^+ / sqrt(k), Q the +-1 signs of
+    gsp_jl_sketch_f64 from the Philox key ``_sampling_seed(seed, 1 << 20)``.  Per block of columns:
+    the right-hand sides Y = D^-1/2 B^T W^1/2 Q^T / sqrt(k) on the device, block CG on the
+    Jacobi-scaled Laplacian D^-1/2 L D^-1/2 (``learning._block_cg``), and the block's share of
+    every R~_e with Z = D^-1/2 U.  Every column of Y is orthogonal to the null space D^1/2 1_c of a
+    component, so the singular systems are consistent; the drift of the solution along that null
+    space is a constant per component in Z, which cancels in Z_u - Z_v.  Blocks and columns are
+    taken in order: the result is reproducible bit for bit.
+    """
+    import types
+    from . import learning
+    torch = nat.require_cuda()
+    n, dev = Ld.shape[0], Ld.device
+    width = _sketch_width(n, k)
+    # D and the operator come from the weights alone: D = W 1 in float64 (row by row, in order)
+    # and diag(Lhat) = 1, so that Lhat D^1/2 1_c = 0 to rounding.  A stored diagonal that is not
+    # exactly W 1 (a float32 Laplacian) would make Lhat slightly indefinite, and CG diverge.
+    rows, cols = row_ids(Ld.indptr), Ld.indices.long()
+    off = rows != cols
+    w = torch.where(off, -Ld.data, torch.zeros_like(Ld.data))
+    deg = torch.empty(n, dtype=torch.float64, device=dev)
+    _call("gsp_degree_f64", nat.i64(n), Ld.indptr, w, None, None, deg, None)
+    dinv = torch.where(deg > 0, deg.clamp(min=1e-300).rsqrt(), torch.zeros_like(deg))
+    diag = torch.nonzero(deg > 0).flatten()
+    view = types.SimpleNamespace(L=DeviceCSR.from_coo(
+        torch.cat([rows[off], diag]), torch.cat([cols[off], diag]),
+        torch.cat([-dinv[rows[off]] * w[off] * dinv[cols[off]], torch.ones_like(deg[diag])]),
+        Ld.shape))
+    key = _sampling_seed(seed, 1 << 20)
+    ne = int(start.numel())
+    e32 = [x.to(torch.int32).contiguous() for x in (start, end)]
+    R = torch.zeros(ne, dtype=torch.float64, device=dev)
+    Y = torch.empty((n, width), dtype=torch.float64, device=dev)
+    maxiter, patience = _sketch_maxiter(n)
+    for j0 in range(0, k, width):
+        wb = min(width, k - j0)
+        Yb = Y if wb == width else torch.empty((n, wb), dtype=torch.float64, device=dev)
+        _call("gsp_jl_sketch_f64", nat.i64(n), Ld.indptr, Ld.indices, Ld.data, dinv, nat.u64(key),
+              nat.i64(j0), nat.i64(wb), nat.i64(k), Yb)
+        U, _, _ = learning._block_cg(view, 1.0, None, None, Yb, _SKETCH_TOL, maxiter, patience)
+        _call("gsp_jl_accumulate_f64", nat.i64(ne), e32[0], e32[1], U, dinv, nat.i64(wb), R)
+        del U
+    return R
+
+
+def graph_sparsify(M, epsilon, maxiter=10, seed=None, *, resistances="exact", sketch_dim=None):
     r"""Sparsify a graph with Spielman-Srivastava (reduction.py:34-147).
 
     ``M``: a :class:`Graph` (combinatorial Laplacian, else ``NotImplementedError``) or a
@@ -313,8 +398,23 @@ def graph_sparsify(M, epsilon, maxiter=10, seed=None):
     distribution actually sampled); per-edge counts stand for the removed ``stats.itemfreq``; the
     graph keeps its coordinates; a matrix in gives the Laplacian ``D' - W'`` as a SciPy CSR matrix
     out (the reference returns ``-W'`` as a ``lil_matrix``).
+
+    ``resistances`` (an addition the reference does not have): ``'exact'`` (the default) as
+    above, limited by the dense factor's 3 N^2 8 bytes to some 5 10^4 vertices; ``'sketch'``
+    estimates every R_e by the Johnson-Lindenstrauss projection of Spielman-Srivastava, from
+    ``sketch_dim`` = k Laplacian solves (default ``ceil(24 ln N / 0.5^2)``: every estimate within
+    a factor 1 +- 0.5 with high probability, which is all the sampler needs).  The solves are
+    block conjugate gradients on the Jacobi-scaled Laplacian in float64, in blocks of at most 256
+    columns (DESIGN.md section 4.22); the signs come from Philox streams of ``seed``, so the same
+    seed gives the same bits.  Everything after R_e is the same for both.  The sketch needs a
+    symmetric Laplacian with non-negative weights (else ``ValueError``) and reads only its
+    off-diagonal entries, the weights: the degrees are their row sums.
     """
     from .graphs import Graph
+    if resistances not in ("exact", "sketch"):
+        raise ValueError("resistances must be 'exact' or 'sketch', not {!r}.".format(resistances))
+    if sketch_dim is not None and int(sketch_dim) < 1:
+        raise ValueError("sketch_dim must be at least 1, not {}.".format(sketch_dim))
     torch, dev = _ctx()
     is_graph = isinstance(M, Graph)
     if is_graph:
@@ -334,11 +434,19 @@ def graph_sparsify(M, epsilon, maxiter=10, seed=None):
         edge = (rows > cols) & (w >= 1e-10)
         start, end, weights = rows[edge], cols[edge], w[edge].contiguous()
         ne = int(weights.numel())
-        Ainv, _, _ = _laplacian_inverse(Ld)
-        R = torch.empty(ne, dtype=torch.float64, device=dev)
-        e32 = [x.to(torch.int32).contiguous() for x in (start, end)]
-        _call("gsp_edge_resistance_f64", nat.i64(ne), e32[0], e32[1], Ainv, nat.i64(N), R)
-        del Ainv
+        if resistances == "sketch":
+            _check_symmetric(Ld, "The resistance sketch")
+            if bool(((rows != cols) & (w < 0)).any()):
+                raise ValueError("The resistance sketch needs non-negative edge weights (the "
+                                 "Laplacian has a positive off-diagonal entry).")
+            k = _sketch_dim(N) if sketch_dim is None else int(sketch_dim)
+            R = _edge_resistances(Ld, start, end, k, seed)
+        else:
+            Ainv, _, _ = _laplacian_inverse(Ld)
+            R = torch.empty(ne, dtype=torch.float64, device=dev)
+            e32 = [x.to(torch.int32).contiguous() for x in (start, end)]
+            _call("gsp_edge_resistance_f64", nat.i64(ne), e32[0], e32[1], Ainv, nat.i64(N), R)
+            del Ainv
         x = weights * torch.clamp(R, min=0)
         xmax = float(x.max().item()) if ne else 0.0
         if not xmax > 0:
