@@ -939,6 +939,41 @@ int gsp_jl_sketch_f64(int64_t n, const int32_t* indptr, const int32_t* indices, 
                       double* Y, void* stream);
 int gsp_jl_accumulate_f64(int64_t ne, const int32_t* erow, const int32_t* ecol, const double* U,
                           const double* dinv, int64_t width, double* R, void* stream);
+/* Kron reduction by random walks (kron_reduction(method='walks'), csrc/schur_walk.cu): the
+ * Schur complement sampler of Durfee, Kyng, Peebles, Rao and Sachdeva.  M (n x n, canonical
+ * float64 CSR, symmetric) has weights w_uv = -M_uv (u != v) and excess e_u, an edge to one ground
+ * vertex g; slot as above (only its sign is read: < 0 kept, >= 0 removed).
+ * gsp_walk_prep_f64: prefix[k] (nnz) := inclusive sum of the weights of row u up to entry k, in
+ *   CSR order (the diagonal entry adds 0); total[u] := the row's sum; excess[u] := excess_in[u]
+ *   when excess_in is not NULL, else M_uu - total[u]; negative excesses are stored as 0.  *status
+ *   (device) gets bit 1 for a positive off-diagonal entry and, without excess_in, bit 2 for an
+ *   excess below -1e-12 M_uu.  status is or-ed into, never cleared.
+ * gsp_schur_walk_f64: items (edge e) x samples for the n_edges edges (eu[e], ev[e]) of weight
+ *   ew[e], item e samples + r, then (ground edge of the removed vertex gu[j]) x samples.  An item
+ *   walks from eu (gu) until a kept vertex or g, then from ev until a kept vertex or g, R summing
+ *   1/w over the steps of the first walk, then 1/ew[e] (1/excess[gu[j]]), then the second walk's
+ *   steps.  Draws: curand_init(key, item, 0); step t of the item (counted over both walks) uses
+ *   words 2 (t mod 2) (lo) and 2 (t mod 2) + 1 (hi) of the (t div 2)-th curand4,
+ *   U = (((hi << 32) | lo) >> 11) 2^-53, X = U (total[x] + excess[x]): the ground when
+ *   X >= total[x] and excess[x] > 0, else the first entry of row x with prefix > X (the last
+ *   positive weight when there is none).  With endpoints c1 != c2 (kept indices) and
+ *   val = 1 / (R samples), an edge item writes rows / cols / vals[4 item .. 4 item + 4) =
+ *   (c1, c2, -val), (c2, c1, -val), (c1, c1, val), (c2, c2, val); with one endpoint g and the
+ *   other c, (c, c, val) at 4 item and three empty slots; a ground item writes one slot at
+ *   4 n_edges samples + (item - n_edges samples).  An empty slot has row = col = -1.  An item
+ *   that needs more than max_steps steps emits nothing and sets bit 4 of *status.  steps (may be
+ *   NULL) gets each item's number of steps.  Needs (n_edges + n_ground) samples and
+ *   (4 n_edges + n_ground) samples below 2^31.
+ */
+int gsp_walk_prep_f64(int64_t n, const int32_t* indptr, const int32_t* indices, const double* data,
+                      const double* excess_in, double* prefix, double* total, double* excess,
+                      int32_t* status, void* stream);
+int gsp_schur_walk_f64(const int32_t* indptr, const int32_t* indices, const double* data,
+                       const double* prefix, const double* total, const double* excess,
+                       const int32_t* slot, int64_t n_edges, const int32_t* eu, const int32_t* ev,
+                       const double* ew, int64_t n_ground, const int32_t* gu, int64_t samples,
+                       uint64_t key, int64_t max_steps, int32_t* rows, int32_t* cols,
+                       double* vals, int32_t* steps, int32_t* status, void* stream);
 
 /* ---------------------------------------------------------------- random graphs ---
  * Draws come from Philox4x32-10 streams of `key` (curand_kernel.h) whose subsequence is a chunk

@@ -7,7 +7,8 @@ interpolation -- and runs on the CUDA engine through :class:`pygsp_b200.filters.
 The multiresolution sequence itself runs on the device too (DESIGN.md section 4.11):
 ``graph_multiresolution`` (largest-eigenvector down-sampling by Chebyshev-filtered subspace
 iteration), :func:`kron_reduction` (independent Schur blocks per component of the removed
-vertices, csrc/schur.cu) and :func:`graph_sparsify` (effective resistances from one float64
+vertices, csrc/schur.cu, or random-walk samples of the Schur complement that never form a dense
+block, csrc/schur_walk.cu and DESIGN.md section 4.23) and :func:`graph_sparsify` (effective resistances from one float64
 factor or, past its size, from a Johnson-Lindenstrauss sketch solved by block CG, csrc/resistance.cu
 and DESIGN.md section 4.22; seeded Philox sampling).  :func:`tree_multiresolution` (reduction.py:633-787, which
 cannot run in the reference) coarsens a tree to its even-depth vertices level after level: the
@@ -67,27 +68,30 @@ def _call(name, *args):
     nat.call(name, *args, nat.stream_ptr())
 
 
-def _schur(M, ind, small_max=None):
-    """Kron reduction of the symmetric float64 DeviceCSR M onto the vertices ``ind`` (host int64
-    array, distinct), as a canonical float64 DeviceCSR in the order of ``ind``.
-
-    M_red - sum_S M_BS M_SS^-1 M_SB over the connected components S of the removed vertices
-    (B: S's kept neighbours): every component is an independent block (csrc/schur.cu).
-    ``small_max`` overrides SMALL_MAX (tests compare the two paths on the same components).
-    """
+def _split(M, ind):
+    """(slot, rem, R, r_rows) of the kept vertices ``ind`` (host int64, distinct) of the float64
+    DeviceCSR M: slot[v] = -1 - (index of v in ind) for a kept vertex, 0 for a removed one (int32);
+    rem the removed vertices, ascending (int32); R, r_rows = M.induced(ind), unsorted triplets of
+    M[ind][:, ind]."""
     torch = nat.require_cuda()
     dev, n, m = M.device, M.shape[0], len(ind)
-    small_max = SMALL_MAX if small_max is None else int(small_max)
     keep = torch.from_numpy(np.ascontiguousarray(ind, dtype=np.int32)).to(dev)
     slot = torch.zeros(n, dtype=torch.int32, device=dev)
     slot[keep.long()] = -1 - torch.arange(m, dtype=torch.int32, device=dev)
     rem = torch.nonzero(slot == 0).flatten().to(torch.int32)
-    R, r_rows = M.induced(keep)        # unsorted triplets: summed with the blocks' by one sort
-    nr = int(rem.numel())
-    if nr == 0:
-        return DeviceCSR.from_coo(r_rows, R.indices, R.data, (m, m))
+    R, r_rows = M.induced(keep)
+    return slot, rem, R, r_rows
 
-    # components of the removed vertices, listed component by component
+
+def _removed_components(M, slot, rem, m):
+    """Connected components of the removed vertices ``rem`` (non-empty) of M and the kept
+    neighbours of each: (nc, cvert, cptr, sizes, comp_of, bidx, nbs, bptr).  cvert lists the
+    removed vertices component by component, component c at cvert[cptr[c] .. cptr[c + 1]) (int32);
+    sizes its sizes and comp_of[v] the component of v, -1 for a kept vertex (int64); its kept
+    neighbours, in increasing kept index, at bidx[bptr[c] .. bptr[c + 1]) (int32, bptr int64),
+    nbs = their numbers.  slot[v] of a removed vertex becomes its position in its component."""
+    torch = nat.require_cuda()
+    dev, n, nr = M.device, M.shape[0], int(rem.numel())
     S, _ = M.induced(rem, increasing=True)
     labels = torch.empty(nr, dtype=torch.int32, device=dev)
     _call("gsp_cc_labels_f64", nat.i64(nr), S.indptr, S.indices, S.data, nat.i32(0), labels, None)
@@ -112,6 +116,25 @@ def _schur(M, ind, small_max=None):
     nbs = torch.bincount(bcomp, minlength=nc)
     bptr = torch.zeros(nc + 1, dtype=torch.int64, device=dev)
     bptr[1:] = torch.cumsum(nbs, 0)
+    return nc, cvert, cptr, sizes, comp_of, bidx, nbs, bptr
+
+
+def _schur(M, ind, small_max=None):
+    """Kron reduction of the symmetric float64 DeviceCSR M onto the vertices ``ind`` (host int64
+    array, distinct), as a canonical float64 DeviceCSR in the order of ``ind``.
+
+    M_red - sum_S M_BS M_SS^-1 M_SB over the connected components S of the removed vertices
+    (B: S's kept neighbours): every component is an independent block (csrc/schur.cu).
+    ``small_max`` overrides SMALL_MAX (tests compare the two paths on the same components).
+    """
+    torch = nat.require_cuda()
+    dev, m = M.device, len(ind)
+    small_max = SMALL_MAX if small_max is None else int(small_max)
+    slot, rem, R, r_rows = _split(M, ind)
+    nr = int(rem.numel())
+    if nr == 0:
+        return DeviceCSR.from_coo(r_rows, R.indices, R.data, (m, m))
+    nc, cvert, cptr, sizes, _, bidx, nbs, bptr = _removed_components(M, slot, rem, m)
     out_len = nbs * nbs
     out_off = torch.zeros(nc + 1, dtype=torch.int64, device=dev)
     out_off[1:] = torch.cumsum(out_len, 0)
@@ -186,6 +209,98 @@ def _check_symmetric(M, what="Kron reduction"):
         raise ValueError("{} on the device needs a symmetric matrix.".format(what))
 
 
+# Kron reduction by random walks (csrc/schur_walk.cu, DESIGN.md section 4.23): bits of its status
+_WALK_NEGATIVE, _WALK_NOT_DOMINANT, _WALK_CAPPED = 1, 2, 4
+_KRON_METHODS = ("exact", "walks")
+_WALK_MAX_STEPS = 2 ** 20
+
+
+def _check_kron_method(method, samples, max_steps=1):
+    if method not in _KRON_METHODS:
+        raise ValueError("method must be 'exact' or 'walks', not {!r}.".format(method))
+    if int(samples) < 1:
+        raise ValueError("samples must be at least 1, not {}.".format(samples))
+    if int(max_steps) < 1:
+        raise ValueError("max_steps must be at least 1, not {}.".format(max_steps))
+
+
+def _schur_walks(M, ind, samples, key, max_steps, excess=None, stats=None):
+    """Kron reduction of the symmetric float64 DeviceCSR M onto the vertices ``ind`` (host int64
+    array, distinct) by random-walk samples of the Schur complement, as a canonical float64
+    DeviceCSR in the order of ``ind`` (csrc/schur_walk.cu).
+
+    M is read as weights w_uv = -M_uv and an excess per vertex, an edge to a ground vertex:
+    ``excess`` (a float64 device tensor, one value per vertex) or, when None, M_uu - sum_v w_uv,
+    which must not fall below -1e-12 M_uu.  Every kept-kept edge and the excess of every kept vertex
+    are exact samples; every other edge and the excess of every removed vertex are sampled
+    ``samples`` times with the Philox key ``key``.  Components of the removed vertices without a
+    kept neighbour contribute nothing and are not walked.  With nothing removed the result is
+    M[ind][:, ind].  ``stats`` (a dict) receives the number of steps of every item ('steps').
+    """
+    torch = nat.require_cuda()
+    dev, n, m = M.device, M.shape[0], len(ind)
+    prefix = torch.empty(M.nnz, dtype=torch.float64, device=dev)
+    total = torch.empty(n, dtype=torch.float64, device=dev)
+    ex = torch.empty(n, dtype=torch.float64, device=dev)
+    status = torch.zeros(1, dtype=torch.int32, device=dev)
+    _call("gsp_walk_prep_f64", nat.i64(n), M.indptr, M.indices, M.data, excess, prefix, total, ex,
+          status)
+    flags = int(status.item())
+    if flags & _WALK_NEGATIVE:
+        raise ValueError("Kron reduction by random walks needs non-negative weights (the matrix "
+                         "has a positive off-diagonal entry).")
+    if flags & _WALK_NOT_DOMINANT:
+        raise ValueError("Kron reduction by random walks needs a diagonally dominant matrix "
+                         "(some M_uu - sum_v |M_uv| is below -1e-12 M_uu).")
+    slot, rem, R, r_rows = _split(M, ind)
+    if rem.numel() == 0:
+        return DeviceCSR.from_coo(r_rows, R.indices, R.data, (m, m))
+    _, _, _, _, comp_of, _, nbs, _ = _removed_components(M, slot, rem, m)
+    dead = (comp_of >= 0) & (nbs[comp_of.clamp(min=0)] == 0)
+
+    # items: the sampled edges (lower triangle, CSR order) and the ground edges of removed vertices
+    rows, cols = row_ids(M.indptr), M.indices.long()
+    removed = slot >= 0
+    sampled = (rows > cols) & (removed[rows] | removed[cols]) & ~dead[rows]
+    eu, ev = rows[sampled].to(torch.int32), cols[sampled].to(torch.int32)
+    ew = (-M.data[sampled]).contiguous()
+    gu = torch.nonzero(removed & ~dead & (ex > 0)).flatten().to(torch.int32)
+    ne, ng = int(eu.numel()), int(gu.numel())
+
+    # exact samples: every kept-kept edge as its Laplacian triplets, and the kept excesses
+    kr, kc = r_rows.long(), R.indices.long()
+    off = kr != kc
+    kex = ex[torch.from_numpy(np.ascontiguousarray(ind, dtype=np.int64)).to(dev)]
+    kx = torch.nonzero(kex > 0).flatten()
+    x_rows = torch.cat([kr[off], kr[off], kx]).to(torch.int32)
+    x_cols = torch.cat([kc[off], kr[off], kx]).to(torch.int32)
+    x_vals = torch.cat([R.data[off], -R.data[off], kex[kx]])
+    slots = (4 * ne + ng) * samples
+    if (ne + ng) * samples >= 2 ** 31 or slots + int(x_rows.numel()) >= 2 ** 31:
+        raise ValueError("The sampled Kron reduction would have {} items and {} entries before "
+                         "summation; at most 2^31 - 1 are supported.".format(
+                             (ne + ng) * samples, slots + int(x_rows.numel())))
+    rows_out = torch.empty(slots, dtype=torch.int32, device=dev)
+    cols_out = torch.empty(slots, dtype=torch.int32, device=dev)
+    vals_out = torch.empty(slots, dtype=torch.float64, device=dev)
+    steps = (torch.empty((ne + ng) * samples, dtype=torch.int32, device=dev)
+             if stats is not None else None)
+    _call("gsp_schur_walk_f64", M.indptr, M.indices, M.data, prefix, total, ex, slot, nat.i64(ne),
+          eu, ev, ew, nat.i64(ng), gu, nat.i64(samples), nat.u64(key), nat.i64(max_steps),
+          rows_out, cols_out, vals_out, steps, status)
+    if int(status.item()) & _WALK_CAPPED:
+        raise ValueError("Kron reduction by random walks: a walk took max_steps = {} steps "
+                         "without reaching a kept vertex; raise max_steps or use "
+                         "method='exact'.".format(max_steps))
+    if stats is not None:
+        stats["steps"] = steps
+    hit = rows_out >= 0
+    # one sort sums every entry's samples in emission order: (i, j) and (j, i) receive the same
+    # values in the same order, so the result is exactly symmetric
+    return DeviceCSR.from_coo(torch.cat([x_rows, rows_out[hit]]), torch.cat([x_cols, cols_out[hit]]),
+                              torch.cat([x_vals, vals_out[hit]]), (m, m))
+
+
 def _kept_ids(ind, n):
     ind = np.asarray(ind)
     if ind.dtype == bool:
@@ -196,7 +311,33 @@ def _kept_ids(ind, n):
     return ind
 
 
-def kron_reduction(G, ind):
+def _kron_graph(G, ind, method, samples, key, max_steps):
+    """kron_reduction of a Graph onto the kept vertices ``ind``, with the walk key ``key``."""
+    from .graphs import Graph
+    torch = nat.require_cuda()
+    if G.lap_type != "combinatorial":
+        raise NotImplementedError("Unknown reduction for {} Laplacian.".format(G.lap_type))
+    if G.is_directed():
+        raise NotImplementedError("This method only work for undirected graphs.")
+    ind = _kept_ids(ind, G.N)
+    with torch.cuda.device(G.device):
+        M = _device_matrix(G.L, G.device)
+        if method == "walks":
+            # the weights are -offdiag(L) and the excess exactly 0: a float32 graph's stored
+            # diagonal is not exactly W 1
+            L = _schur_walks(M, ind, samples, key, max_steps,
+                             excess=torch.zeros(G.N, dtype=torch.float64, device=G.device))
+        else:
+            L = _schur(M, ind)
+        rows = row_ids(L.indptr)
+        off = rows != L.indices.long()
+        return Graph.from_coo(rows[off], L.indices[off], -L.data[off], len(ind),
+                              lap_type=G.lap_type, dtype=G.dtype, device=G.device,
+                              coords=G.coords[ind] if hasattr(G, "coords") else None,
+                              plotting=G.plotting)
+
+
+def kron_reduction(G, ind, *, method="exact", samples=16, seed=None, max_steps=_WALK_MAX_STEPS):
     r"""Compute the Kron reduction (reduction.py:309-382).
 
     ``G``: a :class:`Graph` with a combinatorial Laplacian, or a symmetric sparse matrix
@@ -211,28 +352,33 @@ def kron_reduction(G, ind):
     underflow in float32 are dropped).  The diagonal of ``L_new`` is dropped, as the reference's
     comment intends; its ``Snew`` correction (reduction.py:366-372) is not reproduced (DESIGN.md
     section 2).
+
+    ``method`` (keyword-only, an addition the reference does not have): ``'exact'`` (the default)
+    as above, or ``'walks'``, which never forms a dense block and so reaches graphs whose removed
+    components are too large for one (DESIGN.md section 4.23).  It samples the Schur complement
+    by random walks (Durfee, Kyng, Peebles, Rao and Sachdeva): every edge with a removed end, and
+    the excess ``M_uu - sum_v |M_uv|`` of every removed vertex (an edge to a ground vertex), is
+    walked ``samples`` times from both ends to the kept vertices, and the walks' endpoints get an
+    edge of weight ``1 / (samples * sum of 1/w over the steps)``.  The expected result is the exact
+    reduction; ``samples`` trades entries for variance (16: a spectrum within about +-12 % on
+    k-NN graphs, with several times fewer entries than the exact level).  The draws come from
+    Philox streams of ``seed`` (None means 0): the same seed gives the same bits.  The matrix
+    must be symmetric with non-negative weights and diagonally dominant (excesses below
+    ``-1e-12 M_uu`` raise ``ValueError``; smaller ones count as 0); a graph's weights are read
+    from ``-offdiag(L)`` with no excess.  A walk longer than ``max_steps`` steps raises
+    ``ValueError``.  The matrix branch then returns the sampled ``L_new`` with its diagonal.
     """
     from .graphs import Graph
-    torch = nat.require_cuda()
+    _check_kron_method(method, samples, max_steps)
+    key = _sampling_seed(seed, 1 << 21)
     if isinstance(G, Graph):
-        if G.lap_type != "combinatorial":
-            raise NotImplementedError("Unknown reduction for {} Laplacian.".format(G.lap_type))
-        if G.is_directed():
-            raise NotImplementedError("This method only work for undirected graphs.")
-        ind = _kept_ids(ind, G.N)
-        with torch.cuda.device(G.device):
-            L = _schur(_device_matrix(G.L, G.device), ind)
-            rows = row_ids(L.indptr)
-            off = rows != L.indices.long()
-            Gnew = Graph.from_coo(rows[off], L.indices[off], -L.data[off], len(ind),
-                                  lap_type=G.lap_type, dtype=G.dtype, device=G.device,
-                                  coords=G.coords[ind] if hasattr(G, "coords") else None,
-                                  plotting=G.plotting)
-        return Gnew
+        return _kron_graph(G, ind, method, int(samples), key, int(max_steps))
     _, dev = _ctx()
     M = _device_matrix(G, dev)
     _check_symmetric(M)
     ind = _kept_ids(ind, M.shape[0])
+    if method == "walks":
+        return _schur_walks(M, ind, int(samples), key, int(max_steps)).to_scipy().astype(np.float64)
     return _schur(M, ind).to_scipy().astype(np.float64)
 
 
@@ -483,7 +629,8 @@ def graph_sparsify(M, epsilon, maxiter=10, seed=None, *, resistances="exact", sk
 
 def graph_multiresolution(G, levels, sparsify=True, sparsify_eps=None,
                           downsampling_method="largest_eigenvector", reduction_method="kron",
-                          compute_full_eigen=False, reg_eps=0.005, *, seed=0):
+                          compute_full_eigen=False, reg_eps=0.005, *, seed=0,
+                          kron_method="exact", kron_samples=16, resistances="exact"):
     r"""Compute a pyramid of graphs by Kron reduction (reduction.py:196-306).
 
     Per level: the eigenvector ``V`` of the largest eigenvalue of L (``G._largest_eigenvector``,
@@ -494,7 +641,18 @@ def graph_multiresolution(G, levels, sparsify=True, sparsify_eps=None,
     the level above, ``mr['K_reg']`` (Kron reduction of ``L + reg_eps I``, a SciPy CSR matrix) and
     ``mr['green_kernel']``, as in the reference.  ``seed`` seeds the eigenvector solver and the
     sparsification of every level.
+
+    Keyword-only additions: ``kron_method`` (``'exact'`` or ``'walks'``) and ``kron_samples`` select
+    the reduction of every level and of ``mr['K_reg']`` (:func:`kron_reduction`'s ``method`` and
+    ``samples``; the walks of level i are keyed from ``seed`` and i, those of its ``K_reg`` apart
+    from them), and ``resistances`` is passed to :func:`graph_sparsify`.  With
+    ``kron_method='walks', resistances='sketch'`` no step forms a dense block or factor, and the
+    pyramid reaches graphs of 10^5 vertices and more (DESIGN.md section 4.23).  The synthesis
+    still inverts the analysis exactly: both use the cached ``K_reg``.
     """
+    _check_kron_method(kron_method, kron_samples)
+    if resistances not in ("exact", "sketch"):
+        raise ValueError("resistances must be 'exact' or 'sketch', not {!r}.".format(resistances))
     if sparsify_eps is None:
         sparsify_eps = min(10.0 / np.sqrt(G.N), 0.3)
     if compute_full_eigen:
@@ -511,18 +669,21 @@ def graph_multiresolution(G, levels, sparsify=True, sparsify_eps=None,
         else:
             raise NotImplementedError("Unknown graph downsampling method.")
         if reduction_method == "kron":
-            Gs.append(kron_reduction(Gs[i], ind))
+            Gs.append(_kron_graph(Gs[i], ind, kron_method, int(kron_samples),
+                                  _sampling_seed(seed, 2000 + i), _WALK_MAX_STEPS))
         else:
             raise NotImplementedError("Unknown graph reduction method.")
         if sparsify and Gs[i + 1].N > 2:
             Gs[i + 1] = graph_sparsify(Gs[i + 1], min(max(sparsify_eps, 2.0 / np.sqrt(Gs[i + 1].N)),
-                                                      1.0), seed=_sampling_seed(seed, 1000 + i))
+                                                      1.0), seed=_sampling_seed(seed, 1000 + i),
+                                     resistances=resistances)
         if compute_full_eigen:
             Gs[i + 1].compute_fourier_basis()
         else:
             Gs[i + 1].estimate_lmax()
         Gs[i + 1].mr = {"idx": ind, "orig_idx": Gs[i].mr["orig_idx"][ind], "level": i}
-        Gs[i].mr["K_reg"] = _kron_regularized(Gs[i], ind, reg_eps)
+        Gs[i].mr["K_reg"] = _kron_regularized(Gs[i], ind, reg_eps, kron_method, int(kron_samples),
+                                              _sampling_seed(seed, 3000 + i))
         Gs[i].mr["_kreg_key"] = (reg_eps, ind.tobytes())
         Gs[i].mr["green_kernel"] = filters.Filter(Gs[i], lambda x: 1.0 / (reg_eps + x))
         Gs[i].mr["_green_eps"] = reg_eps
@@ -653,9 +814,10 @@ def tree_multiresolution(G, Nlevel, reduction_method="resistance_distance",
     return Gs, subsampled_vertex_indices
 
 
-def _kron_regularized(G, ind, reg_eps):
+def _kron_regularized(G, ind, reg_eps, method="exact", samples=16, key=0):
     """Kron reduction of L + reg_eps I onto ind (reduction.py:302-303), L + reg_eps I assembled
-    on the device."""
+    on the device.  ``method='walks'`` samples it with the Philox key ``key``, the excess of every
+    vertex being reg_eps itself (not re-derived from the assembled diagonal)."""
     torch = nat.require_cuda()
     with torch.cuda.device(G.device):
         L = _device_matrix(G.L, G.device)
@@ -666,6 +828,10 @@ def _kron_regularized(G, ind, reg_eps):
                                torch.cat([L.data, torch.full((n,), float(reg_eps),
                                                              dtype=torch.float64,
                                                              device=G.device)]), (n, n))
+        if method == "walks":
+            excess = torch.full((n,), float(reg_eps), dtype=torch.float64, device=G.device)
+            return _schur_walks(M, ind, samples, key, _WALK_MAX_STEPS,
+                                excess=excess).to_scipy().astype(np.float64)
         return _schur(M, ind).to_scipy().astype(np.float64)
 
 
