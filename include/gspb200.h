@@ -733,6 +733,51 @@ GSPB200_DECLARE_NEIGHBOR_API(f64, double)
 GSPB200_DECLARE_LAYOUT_API(f32, float)
 GSPB200_DECLARE_LAYOUT_API(f64, double)
 
+/* ---------------------------------------------------------- Barnes-Hut spring layout ---
+ * The spring layout above with the repulsion sum_j delta_ij k^2 / d_ij^2 replaced by a
+ * Barnes-Hut tree walk (csrc/barnes_hut.cu, DESIGN.md 4.24); dim must be 1, 2 or 3 and theta
+ * finite and >= 0.  The attraction, the move and the arguments shared with gsp_spring_step_* /
+ * gsp_spring_layout_* (including states and fixed) are the same.  Each iteration sorts the
+ * vertices by Morton key (graphs.morton_order's 21 bits per axis), builds Karras's binary radix
+ * tree over the sorted keys, a duplicate key broken by sorted index, and aggregates every node's
+ * count, axis-aligned bounding box (AABB) and centroid.  Vertex x sees a cell of M points with
+ * centroid c, AABB diagonal D and distance rho from x to the AABB as one monopole
+ * M (x - c) / max(|x - c|^2, 0.01^2) when D <= theta rho and rho >= 0.01, or when D = 0;
+ * otherwise the cell is opened, and a single point is summed exactly.  theta = 0 opens every
+ * cell that is not one point.  Results are bit-identical from run to run and card to card.
+ * Device scratch, allocated once per call: (52 + 40 dim) n bytes plus CUB's sort storage,
+ * and 8 dim n more for gsp_spring_layout_bh_* without states (gsp_spring_bh_tree: 8 dim n
+ * less).  Returns
+ * GSP_ERR_UNSUPPORTED if a walk's stack overflowed (it cannot: the tree is at most 94 deep).
+ *
+ * gsp_spring_bh_tree: the tree of one (n, dim) position block, for tests and probes.  Node
+ * numbering (Karras 2012): internal node v (0 <= v < n - 1) covers a contiguous range of sorted
+ * indices; the root is node 0 (for n = 1 the tree is the single leaf).  Caller buffers (device):
+ *   ids        n int32          ids[s] = vertex at sorted index s (stable sort of the keys)
+ *   children   2 (n - 1) int32  left, right child of v: w >= 0 is internal node w, w < 0 the
+ *                               leaf at sorted index ~w
+ *   counts     n - 1 int32      points under v
+ *   boxes      (n - 1) 2 dim    AABB of v's points: lo[dim] then hi[dim]
+ *   centroids  (n - 1) dim      centroid of v's points
+ * For n <= 1 only ids is written.
+ */
+#define GSPB200_DECLARE_BH_API(SUF, T)                                                           \
+  int gsp_spring_step_bh_##SUF(int64_t n, int dim, const int32_t* indptr, const int32_t* indices, \
+                               const T* data, double k, double t, const uint8_t* fixed,          \
+                               const double* pos_in, double* pos_out, double theta,              \
+                               void* stream);                                                    \
+  int gsp_spring_layout_bh_##SUF(int64_t n, int dim, const int32_t* indptr,                      \
+                                 const int32_t* indices, const T* data, double k,                \
+                                 int iterations, const double* temps_host,                       \
+                                 const uint8_t* fixed, double* pos, double* states,              \
+                                 double theta, void* stream);
+
+GSPB200_DECLARE_BH_API(f32, float)
+GSPB200_DECLARE_BH_API(f64, double)
+
+int gsp_spring_bh_tree(int64_t n, int dim, const double* pos, int32_t* ids, int32_t* children,
+                       int32_t* counts, double* boxes, double* centroids, void* stream);
+
 #define GSPB200_DECLARE_GRAPH_API(SUF, T)                                                        \
   int gsp_csr_inspect_##SUF(int64_t n, const int32_t* indptr, const int32_t* indices,            \
                             const T* data, int64_t* stats_dev, void* stream);                    \

@@ -10,7 +10,7 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 OUT_DIR = os.path.join(HERE, "_lib")
 LIB = os.path.join(OUT_DIR, "libgspb200.so")
-SOURCES = ["runtime.cu", "cheby.cu", "cheby_bank.cu", "cheby_tiled.cu", "pair_plan.cu", "graph.cu", "lanczos.cu", "halo.cu", "generate.cu", "staging.cu", "dist.cu", "cg.cu", "block.cu", "difference.cu", "connectivity.cu", "krylov.cu", "moments.cu", "schur.cu", "simplex.cu", "neighbors.cu", "layout.cu", "tv.cu", "random_graphs.cu", "random_regular.cu", "structured.cu", "tree.cu", "resistance.cu", "schur_walk.cu"]
+SOURCES = ["runtime.cu", "cheby.cu", "cheby_bank.cu", "cheby_tiled.cu", "pair_plan.cu", "graph.cu", "lanczos.cu", "halo.cu", "generate.cu", "staging.cu", "dist.cu", "cg.cu", "block.cu", "difference.cu", "connectivity.cu", "krylov.cu", "moments.cu", "schur.cu", "simplex.cu", "neighbors.cu", "layout.cu", "tv.cu", "random_graphs.cu", "random_regular.cu", "structured.cu", "tree.cu", "resistance.cu", "schur_walk.cu", "barnes_hut.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 

@@ -11,6 +11,16 @@ layout draws the reference's seeded start on the host, runs every iteration on t
 (``gsp_spring_layout_*``, csrc/layout.cu: an all-pairs float64 kernel) at the reference's exact
 temperatures, and rescales the result on the host with the reference's operations.
 
+``set_coordinates('spring', repulsion='barnes_hut', theta=0.5)`` replaces only the repulsion sum,
+which costs O(N^2) per iteration, by a Barnes-Hut walk of a Morton-ordered radix tree rebuilt on
+the device every iteration (``gsp_spring_layout_bh_*``, csrc/barnes_hut.cu, DESIGN.md section
+4.24): O(N log N), for dim 1, 2 or 3.  A cell is taken as one monopole when the diagonal of its
+points' bounding box is at most ``theta`` times the distance from the vertex to that box (and the
+distance is at least 0.01), so each vertex's repulsion is within a proven bound of the exact sum
+(DESIGN.md section 4.24); ``theta=0`` opens every cell of distinct points.  The attraction,
+the move, the cooling schedule, ``fixed``, ``pos``, ``k``, the seeded start and the rescale are
+unchanged, and ``repulsion='exact'``, the default, is the all-pairs kernel.
+
 Differences from the reference (DESIGN.md section 2): the spring layout's float64 sums run in
 another order (the iteration is chaotic, so a 50-iteration layout differs from the reference's
 by more than rounding, while each single step agrees to rounding); the sign of each eigenmap
@@ -39,7 +49,15 @@ class LayoutMixIn:
         kwargs : dict
             Arguments of the Fruchterman-Reingold layout when kind is 'spring': ``dim`` (2),
             ``k`` (None: sqrt(1/N)), ``pos`` (None), ``fixed`` ([]), ``iterations`` (50),
-            ``scale`` (1.0) and ``center`` (None: the origin).
+            ``scale`` (1.0) and ``center`` (None: the origin).  Two more select the repulsion
+            sum: ``repulsion`` ('exact', the default: all pairs, O(N^2) per iteration; or
+            'barnes_hut': a Barnes-Hut tree walk, O(N log N), approximate within a proven
+            bound, dim 1, 2 or 3 only) and ``theta`` (0.5; 'barnes_hut' only: a cell is one
+            monopole when its bounding box's diagonal is at most ``theta`` times its distance
+            from the vertex, so a smaller ``theta`` is slower and closer to the exact sum).
+            An unknown ``repulsion``, ``theta`` with 'exact', a negative or non-finite
+            ``theta``, and a ``dim`` other than 1, 2, 3 or a non-finite ``pos`` with
+            'barnes_hut' raise ``ValueError``.
         """
         if not isinstance(kind, str):
             coords = np.asanyarray(kind).squeeze()
@@ -96,8 +114,9 @@ class LayoutMixIn:
         return info["com_coords"][node_com] + comm_rad[:, None] * offset
 
     def _fruchterman_reingold(self, dim=2, k=None, pos=None, fixed=[], iterations=50,
-                              scale=1.0, center=None, seed=None):
+                              scale=1.0, center=None, seed=None, repulsion="exact", theta=None):
         """The reference's argument handling (_layout.py:136-166) around the device layout."""
+        _repulsion_theta(repulsion, theta, dim)
         if center is None:
             center = np.zeros((1, dim))
         if np.shape(center)[1] != dim:
@@ -119,7 +138,7 @@ class LayoutMixIn:
         if k is None:
             k = np.sqrt(1.0 / self.N)
 
-        pos = _spring_layout(self, start, k, iterations, fixed)
+        pos = _spring_layout(self, start, k, iterations, fixed, repulsion=repulsion, theta=theta)
         if len(fixed) == 0:
             pos = _rescale_layout(pos, scale=scale) + center
         return pos
@@ -136,41 +155,72 @@ def _temperatures(iterations):
     return np.array(out, dtype=np.float64)
 
 
-def _spring_inputs(G, pos, fixed):
+def _repulsion_theta(repulsion, theta, dim):
+    """The ``theta`` of a Barnes-Hut repulsion (0.5 by default), None for the exact one; raises
+    ``ValueError`` on an unknown ``repulsion``, a ``theta`` given with 'exact', a negative or
+    non-finite ``theta`` and a Barnes-Hut ``dim`` other than 1, 2, 3."""
+    if repulsion == "exact":
+        if theta is not None:
+            raise ValueError("theta applies only to repulsion='barnes_hut'.")
+        return None
+    if repulsion != "barnes_hut":
+        raise ValueError("Unexpected argument repulsion=%r: 'exact' or 'barnes_hut'." % (repulsion,))
+    theta = 0.5 if theta is None else float(theta)
+    if not (np.isfinite(theta) and theta >= 0):
+        raise ValueError("theta must be finite and >= 0, got %r." % (theta,))
+    if dim not in (1, 2, 3):
+        raise ValueError("repulsion='barnes_hut' takes dim 1, 2 or 3, got %r." % (dim,))
+    return theta
+
+
+def _spring_inputs(G, pos, fixed, repulsion="exact", theta=None):
+    pos = np.ascontiguousarray(pos, dtype=np.float64)
+    theta = _repulsion_theta(repulsion, theta, pos.shape[1] if pos.ndim == 2 else None)
+    if theta is not None and not np.isfinite(pos).all():
+        raise ValueError("repulsion='barnes_hut' needs finite start positions.")
     torch = nat.require_cuda()
-    pos = torch.as_tensor(np.ascontiguousarray(pos, dtype=np.float64), device=G.device)
+    pos = torch.as_tensor(pos, device=G.device)
     mask = None
     if len(fixed) > 0:
         mask = np.isin(np.arange(G.N), np.asarray(list(fixed))).astype(np.uint8)
         mask = torch.as_tensor(mask, device=G.device)
-    return torch, pos.contiguous(), mask
+    return torch, pos.contiguous(), mask, theta
 
 
-def _spring_layout(G, start, k, iterations, fixed, keep_states=False):
+def _spring_layout(G, start, k, iterations, fixed, keep_states=False, *, repulsion="exact",
+                   theta=None):
     """``iterations`` spring iterations on the device from ``start`` (N, dim).  Returns the final
     positions (host float64), and with ``keep_states`` also the (iterations, N, dim) positions
-    after every iteration."""
-    torch, pos, mask = _spring_inputs(G, start, fixed)
+    after every iteration.  ``repulsion`` and ``theta`` are those of ``set_coordinates``."""
+    torch, pos, mask, theta = _spring_inputs(G, start, fixed, repulsion, theta)
     n, dim = pos.shape
     temps = _temperatures(int(iterations))
     states = None
     if keep_states:
         states = torch.empty((len(temps), n, dim), dtype=torch.float64, device=G.device)
     W = G.W
-    G._call("gsp_spring_layout", nat.i64(n), nat.i32(dim), W.indptr, W.indices, W.data,
-            nat.f64(k), nat.i32(len(temps)), temps, mask, pos, states)
+    args = (nat.i64(n), nat.i32(dim), W.indptr, W.indices, W.data, nat.f64(k),
+            nat.i32(len(temps)), temps, mask, pos, states)
+    if theta is None:
+        G._call("gsp_spring_layout", *args)
+    else:
+        G._call("gsp_spring_layout_bh", *args, nat.f64(theta))
     out = pos.cpu().numpy()
     return (out, states.cpu().numpy()) if keep_states else out
 
 
-def _spring_step(G, pos, k, t, fixed=()):
+def _spring_step(G, pos, k, t, fixed=(), *, repulsion="exact", theta=None):
     """One spring iteration at temperature ``t`` from the positions ``pos`` (N, dim) on the
     device; returns the new positions (host float64)."""
-    torch, cur, mask = _spring_inputs(G, pos, fixed)
+    torch, cur, mask, theta = _spring_inputs(G, pos, fixed, repulsion, theta)
     nxt = torch.empty_like(cur)
     W = G.W
-    G._call("gsp_spring_step", nat.i64(cur.shape[0]), nat.i32(cur.shape[1]), W.indptr, W.indices,
-            W.data, nat.f64(k), nat.f64(t), mask, cur, nxt)
+    args = (nat.i64(cur.shape[0]), nat.i32(cur.shape[1]), W.indptr, W.indices, W.data,
+            nat.f64(k), nat.f64(t), mask, cur, nxt)
+    if theta is None:
+        G._call("gsp_spring_step", *args)
+    else:
+        G._call("gsp_spring_step_bh", *args, nat.f64(theta))
     return nxt.cpu().numpy()
 
 
